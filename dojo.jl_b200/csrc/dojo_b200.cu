@@ -406,7 +406,8 @@ extern "C" int dojo_create(const DojoMechanismDesc* d, int device, int max_batch
     P.ncol = 12 * Nb + nu;
     for (int j = 0; j < Ne; ++j)
       for (int k = 0; k < joints[j].nfree_t + joints[j].nfree_r; ++k) { ucol.push_back(j); ucol.push_back(k); }
-    for (int pass = 0; pass < 4; ++pass) {
+    // every warp solves ch / nw columns of a chunk (dojo_grad.cuh gradients()), so the chunk never gets narrower than nw
+    for (int pass = 0; pass < 4 && (32 >> pass) >= nw; ++pass) {
       P.ch = 32 >> pass;  // 32, 16, 8, 4 columns per chunk
       int g = P.arena_len;
       for (int b = 0; b < Nb; ++b) { bodies[b].gb_off = g; g += 30; }

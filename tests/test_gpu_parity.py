@@ -31,15 +31,18 @@ MAX_PATH_FLIPS = 0.002
 
 
 def _contact_modes(mech, sol):
-    off = mech.contact_sol_offset(0) if mech.Ni else 0
-    s = sol[:, off:].reshape(sol.shape[0], mech.Ni, 8)
-    return s[:, :, 4] > s[:, :, 0]
+    """gamma_1 > s_1 per contact: a contact's entry is [s(N/2); gamma(N/2)] for every model, normal component first"""
+    idx = np.array([mech.contact_sol_offset(c) for c in range(mech.Ni)], dtype=int)
+    half = np.array([c.dim // 2 for c in mech.contacts], dtype=int)
+    return sol[:, idx + half] > sol[:, idx]
 
 
-def _compare_rollout(name, B, T, seed, scale, opts=None, max_mismatch=0.01, tol_same=TOL_SAME_PATH, tol_all=TOL_SOLVER):
+def _compare_rollout(name, B, T, seed, scale, opts=None, max_mismatch=0.01, tol_same=TOL_SAME_PATH, tol_all=TOL_SOLVER, tol_median=None):
+    """`name`: a mechanism name or a Mechanism.  tol_median: optional bound on the median same-iteration error."""
     from dojo_jl_b200.solver import BatchedStepper
     from oracle.oracle import Oracle
-    mech = dj.get_mechanism(name)
+    mech = dj.get_mechanism(name) if isinstance(name, str) else name
+    name = mech.name
     rng = np.random.default_rng(seed)
     Z = jittered_states(mech, B, rng) if mech.Nb > 1 else np.tile(mech.z0, (B, 1))
     stepper = BatchedStepper(mech, B)
@@ -90,6 +93,8 @@ def _compare_rollout(name, B, T, seed, scale, opts=None, max_mismatch=0.01, tol_
     assert mismatched <= max_mismatch * total, f"{name}: {mismatched}/{total} environments took a different iteration count"
     assert path_flips <= max(1, MAX_PATH_FLIPS * total), f"{name}: {path_flips}/{total} environments left the oracle's path"
     assert np.quantile(same_errs, 0.99) <= TOL_SAME_Q99, f"{name}: 99 % quantile of the same-iteration error {np.quantile(same_errs, 0.99)}"
+    if tol_median is not None:
+        assert np.median(same_errs) <= tol_median, f"{name}: median same-iteration error {np.median(same_errs)}"
     return mismatched, total
 
 
