@@ -34,6 +34,8 @@ Deviations (documented switches, SURVEY.md Appendix D):
     never fire -- candidate_step! clips |w|^2 to (3.9/h^2)^2 / |w|^2 < 3.9/h^2 before line_search! compares it with 3.91/h^2
     (DESIGN.md section 6) -- so no path produces it; _check_single keeps the mapping to the reference's error().
 """
+import math
+import warnings
 from typing import Callable, Optional
 
 import numpy as np
@@ -63,15 +65,68 @@ def _check_single(status):
         raise RuntimeError("Excessive angular velocity.")  # reference: error(...) in line_search!
 
 
+def _scn(a: float) -> str:
+    """scn(a, digits=0) (utilities/methods.jl:9-43): one significant digit and the exponent, e.g. ' 4e-5'."""
+    a = float(a)
+    if math.isnan(a):
+        return " NaN "
+    if a == math.inf:
+        return " Inf"
+    if a == -math.inf:
+        return "-Inf"
+    if a == 0:
+        e, m = 0, 0.0
+    else:
+        e = int(math.floor(math.log(abs(a)) / math.log(10)))
+        m = a * math.exp(-e * math.log(10))
+    m = float(round(m))  # Julia's round: to nearest, ties to even, like Python's
+    if m == 10.0:
+        m, e = 1.0, e + 1
+    sgn = " " if a >= 0 else ""
+    return f"{sgn}{int(math.floor(m))}e{'+' if e >= 0 else '-'}{abs(e)}"
+
+
+def format_solver_trace(trace) -> str:
+    """The table mehrotra! prints with SolverOptions(verbose = true) (solver_header / solver_status, solver/mehrotra.jl:75-98) for one
+    solve, from its trace [max_iter, 5] (BatchedStepper.step(..., trace=True)): one line per loop head n, `n  bvio  rvio  α  μ`, where α
+    and μ belong to the iteration before the head.  The reference's last two columns, |res|∞ and |Δ|∞, are left out: there both are
+    norm(full_vector(system), Inf) of the same vector, so they print the same number, and that vector -- the residual assembled at the
+    iterate of the head -- is never formed on the device, which decides convergence from the violations alone."""
+    tr = np.asarray(trace, dtype=float)
+    rows = int(np.count_nonzero(~np.isnan(tr[:, 4]))) if tr.size else 0  # the trials column is NaN exactly in the padding rows
+    lines = [" " * 49, "n    bvio    rvio     α       μ", "–" * 49]
+    for r in range(rows):
+        rvio, bvio, alpha, mu = tr[r, :4]
+        lines.append(f"{r + 1}   {_scn(bvio)}   {_scn(rvio)}   {_scn(alpha)}   {_scn(mu)}")
+    return "\n".join(lines)
+
+
+def _print_trace(trace, status) -> None:
+    print(format_solver_trace(trace))
+    if int(status) == 1:
+        warnings.warn("failed mehrotra")  # solver/mehrotra.jl:31, at the head of the last iteration
+
+
+def _verbose(opts) -> bool:
+    return opts is not None and bool(opts.verbose)
+
+
 def step(mechanism: Mechanism, z, u, opts=None, literal_q1: bool = False, device: int = 0):
     """step!(mechanism, z, u; opts).  z: [13Nb] or [B, 13Nb]; u: [nu] or [B, nu].  Returns z_next (same shape); for a batch
-    also (status, iters)."""
+    also (status, iters).  With opts.verbose and a single environment the step runs traced and prints the solver's table
+    (format_solver_trace) and, when it ends :failed, the warning "failed mehrotra", as mehrotra! does; batched calls do not print
+    (use BatchedStepper.step(..., trace=True) for the traces of a batch)."""
     z = np.asarray(z, dtype=float)
     single = z.ndim == 1
     Z = np.atleast_2d(z)
     U = np.atleast_2d(np.asarray(u, dtype=float))
     s = _stepper(mechanism, Z.shape[0], device)
-    Zn, status, iters = s.step(Z, U, opts, flags=DOJO_FLAG_Q1_LITERAL_RETURN if literal_q1 else 0)
+    flags = DOJO_FLAG_Q1_LITERAL_RETURN if literal_q1 else 0
+    if single and _verbose(opts):
+        Zn, status, iters, tr = s.step(Z, U, opts, flags=flags, trace=True)
+        _print_trace(tr[0], status[0])
+    else:
+        Zn, status, iters = s.step(Z, U, opts, flags=flags)
     if single:
         _check_single(status)
         return Zn[0]
@@ -80,7 +135,9 @@ def step(mechanism: Mechanism, z, u, opts=None, literal_q1: bool = False, device
 
 def simulate(mechanism: Mechanism, steps: int, z0=None, control: Optional[Callable] = None, record: bool = False, opts=None, device: int = 0):
     """simulate!(mechanism, steps, storage, control!): `control(k)` returns the input(s) of step k ([nu] or [B, nu]; None = 0).
-    Returns the final state(s) and, with record=True, the trajectory [steps, B, 13Nb] (the reference's Storage)."""
+    Returns the final state(s) and, with record=True, the trajectory [steps, B, 13Nb] (the reference's Storage).
+    The steps are fused into one launch, except with opts.verbose and a single environment: then every step is its own traced
+    launch and prints its solver table, as simulate! does with verbose = true (same results).  Batched calls do not print."""
     z0 = mechanism.z0 if z0 is None else z0
     z0 = np.asarray(z0, dtype=float)
     single = z0.ndim == 1
@@ -94,8 +151,17 @@ def simulate(mechanism: Mechanism, steps: int, z0=None, control: Optional[Callab
             uk = control(k)
             if uk is not None:
                 U[k] = np.asarray(uk, dtype=float)
-    out = s.rollout(Z, U, steps, opts, record=record)
-    Zf, traj = out[0], (out[2] if record else None)
+    if single and _verbose(opts):
+        traj = np.empty((steps, B, mechanism.nz)) if record else None
+        Zf = Z
+        for k in range(steps):
+            Zf, status, _, tr = s.step(Zf, None if U is None else U[k], opts, trace=True)
+            _print_trace(tr[0], status[0])
+            if record:
+                traj[k] = Zf
+    else:
+        out = s.rollout(Z, U, steps, opts, record=record)
+        Zf, traj = out[0], (out[2] if record else None)
     if single:
         return (Zf[0], traj[:, 0]) if record else Zf[0]
     return (Zf, traj) if record else Zf

@@ -31,6 +31,13 @@ static const void* step_kernel_fn(bool any_contact, bool grad, bool plan_smem) {
   if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return grad ? (const void*)dojo_step_kernel<true, true> : (const void*)dojo_step_kernel<false, true>;
   return grad ? (const void*)dojo_step_kernel<true, false> : (const void*)dojo_step_kernel<false, false>;
 }
+// the traced forward kernel (dojo_step_trace) of the compilation and plan placement step_kernel_fn picks for the untraced one
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_trace_kernel();
+static const void* step_trace_kernel_fn(bool any_contact, bool plan_smem) {
+  if (any_contact) return dojo_cm_step_trace_kernel();
+  if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<false, true, true>;
+  return (const void*)dojo_step_kernel<false, false, true>;
+}
 
 // Order of the work queue.  A per-step launch ends when its slowest environment ends: an environment that stalls (ten line-search
 // trials per iteration up to max_iter, ~6 x the median time) and is dequeued late finishes alone.  Which environments stall is not
@@ -173,6 +180,9 @@ struct DojoHandle {
   bool orthant_contact = false;                   // ... an ImpactContact / LinearContact
   bool tra_joint = false;                         // ... or translational springs / dampers / limits
   const void *k_fwd = nullptr, *k_grad = nullptr;  // dojo_step_kernel<false> / <true> of the compilation that serves this mechanism
+  const void* k_fwd_trace = nullptr;               // its traced variant, set up by the first dojo_step_trace call
+  double* d_trace = nullptr;                       // grow-only device buffer of dojo_step_trace (host-pointer calls)
+  size_t trace_doubles = 0;
   std::string err;
 };
 // [hostemu:handle:end]
@@ -695,7 +705,7 @@ extern "C" int dojo_create(const DojoMechanismDesc* d, int device, int max_batch
 extern "C" int dojo_destroy(DojoHandle* h) {
   if (!h) return DOJO_OK;
   cudaSetDevice(h->device);
-  cudaFree(h->d_key); cudaFree(h->d_order); cudaFree(h->d_prev_iters); cudaFree(h->d_prof); cudaFree(h->d_blob); cudaFree(h->d_counter); cudaFree(h->d_kin_order); cudaFree(h->d_kjws); cudaFree(h->d_kjout); cudaFree(h->d_recZ[0]); cudaFree(h->d_recZ[1]); cudaFree(h->d_recS); cudaFree(h->d_recD); cudaFree(h->d_recAny); cudaFree(h->d_envTheta); cudaFree(h->d_envNorm); cudaFree(h->d_envS); cudaFree(h->d_envSn); cudaFree(h->d_envA); cudaFree(h->d_envR); cudaFree(h->d_envS0); cudaFree(h->d_envDone); cudaFree(h->d_X); cudaFree(h->d_Xn); cudaFree(h->d_gsol); cudaFree(h->d_gstatus); cudaFree(h->d_done);
+  cudaFree(h->d_key); cudaFree(h->d_order); cudaFree(h->d_prev_iters); cudaFree(h->d_prof); cudaFree(h->d_blob); cudaFree(h->d_counter); cudaFree(h->d_kin_order); cudaFree(h->d_kjws); cudaFree(h->d_kjout); cudaFree(h->d_recZ[0]); cudaFree(h->d_recZ[1]); cudaFree(h->d_recS); cudaFree(h->d_recD); cudaFree(h->d_recAny); cudaFree(h->d_envTheta); cudaFree(h->d_envNorm); cudaFree(h->d_envS); cudaFree(h->d_envSn); cudaFree(h->d_envA); cudaFree(h->d_envR); cudaFree(h->d_envS0); cudaFree(h->d_envDone); cudaFree(h->d_X); cudaFree(h->d_Xn); cudaFree(h->d_gsol); cudaFree(h->d_gstatus); cudaFree(h->d_done); cudaFree(h->d_trace);
   for (int k = 0; k < 2; ++k) { cudaFree(h->d_Fz[k]); cudaFree(h->d_Fu[k]); if (h->ev_kernel[k]) cudaEventDestroy(h->ev_kernel[k]); if (h->ev_copy[k]) cudaEventDestroy(h->ev_copy[k]); }
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
   cudaFree(h->d_Z); cudaFree(h->d_U); cudaFree(h->d_F); cudaFree(h->d_Zn); cudaFree(h->d_sol); cudaFree(h->d_status); cudaFree(h->d_iters);
@@ -752,9 +762,10 @@ static Options make_options(const DojoSolverOptions* o) {
 
 static int launch_forward(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ, const double* dU, const double* dFext, double* dZn, double* dsol,
                           double* dsol_raw, int32_t* dstatus, int32_t* diters, uint32_t flags, cudaStream_t s, int* done_count = nullptr, int* done_list = nullptr,
-                          DojoGather* g = nullptr) {
+                          DojoGather* g = nullptr, double* dtrace = nullptr) {
   StepArgs a;
   a.n_peers = 0; a.gather_off = 0;
+  a.trace = dtrace;  // non-null: the traced kernel (dojo_step_trace_async)
   if (g) {
     if (!g->connected || g->h != h || B != g->B) { h->err = "dojo_step_gather_async: gather not connected / made for another handle / B differs from B_local"; return DOJO_EINVAL; }
     a.n_peers = g->world;
@@ -788,7 +799,8 @@ static int launch_forward(DojoHandle* h, const DojoSolverOptions* opts, int B, c
   a.plan_blob = h->d_blob; a.plan_bytes = h->blob_bytes; a.plan_smem_off = h->plan_smem_off; a.plan_smem_bytes = h->plan_smem_bytes; a.plan_smem_mask = h->plan_smem_mask;
   for (int k = 0; k < 8; ++k) a.plan_off[k] = h->blob_off[k];
   int grid = std::min((B + h->slots - 1) / h->slots, h->sm_count * h->envs_per_sm);
-  { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(h->k_fwd, dim3(grid), dim3(32 * h->nw * h->slots), kargs, h->smem_fwd, s)); }
+  const void* k = dtrace ? h->k_fwd_trace : h->k_fwd;
+  { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(k, dim3(grid), dim3(32 * h->nw * h->slots), kargs, h->smem_fwd, s)); }
   CUDA_TRY(h, cudaGetLastError());
   h->launches += 1;
   if (g) g->expected += (unsigned long long)g->world * (unsigned long long)grid;  // every rank launches the same grid (same B_local, same device type)
@@ -836,20 +848,56 @@ static int ensure_staging(DojoHandle* h) {
   return DOJO_OK;
 }
 
-// Host- or device-pointer entry: host buffers are staged through pinned memory, copies are part of the call.
-extern "C" int dojo_step(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* Z, const double* U, const double* Fext, double* Zn,
-                         double* sol, int32_t* status, int32_t* iters, uint32_t flags) {
-  if (!h || B <= 0 || B > h->max_batch || !Z || !Zn) { if (h) h->err = "dojo_step: bad arguments (B must be in 1..max_batch)"; return DOJO_EINVAL; }
+// ---- traced step! (solver/mehrotra.jl verbose mode): dojo_step + one row per loop-head test of the solver (include/dojo_b200.h)
+// The traced kernel is set up on first use, with the shared-memory attributes dojo_create gives k_fwd.
+static int ensure_trace_kernel(DojoHandle* h) {
+  if (h->k_fwd_trace) return DOJO_OK;
+  const void* k = step_trace_kernel_fn(h->any_contact, h->plan_smem_mask == 0xff);
+  int optin = 0;
+  cudaFuncAttributes fa;
+  CUDA_TRY(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+  CUDA_TRY(h, cudaFuncGetAttributes(&fa, k));
+  CUDA_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
+  CUDA_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  h->k_fwd_trace = k;
+  return DOJO_OK;
+}
+
+extern "C" int dojo_step_trace_async(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ, const double* dU, const double* dFext,
+                                     double* dZn, double* dsol, int32_t* dstatus, int32_t* diters, double* dtrace, uint32_t flags, void* cuda_stream) {
+  if (!h || B <= 0 || !dZ || !dZn || !dtrace) { if (h) h->err = "dojo_step_trace_async: bad arguments (trace is required)"; return DOJO_EINVAL; }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  int rc = ensure_trace_kernel(h);
+  if (rc != DOJO_OK) return rc;
+  return launch_forward(h, opts, B, dZ, dU, dFext, dZn, dsol, nullptr, dstatus, diters, flags, (cudaStream_t)cuda_stream, nullptr, nullptr, nullptr, dtrace);
+}
+
+// Host- or device-pointer entry of dojo_step and, with a trace buffer, dojo_step_trace: host buffers are staged through pinned memory,
+// copies are part of the call.
+static int step_sync(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* Z, const double* U, const double* Fext, double* Zn,
+                     double* sol, int32_t* status, int32_t* iters, double* trace, uint32_t flags) {
   CUDA_TRY(h, cudaSetDevice(h->device));
   const Plan& P = h->plan;
+  auto launch = [&](const double* dZ, const double* dU, const double* dF, double* dZn, double* dsol, int32_t* dst, int32_t* dit, double* dtr,
+                    cudaStream_t s) {
+    return trace ? dojo_step_trace_async(h, opts, B, dZ, dU, dF, dZn, dsol, dst, dit, dtr, flags, s)
+                 : dojo_step_async(h, opts, B, dZ, dU, dF, dZn, dsol, dst, dit, flags, s);
+  };
   if (is_device_ptr(Z)) {  // resident data: launch on the handle's stream and wait
-    int rc = dojo_step_async(h, opts, B, Z, U, Fext, Zn, sol, status, iters, flags, h->stream);
+    int rc = launch(Z, U, Fext, Zn, sol, status, iters, trace, h->stream);
     if (rc != DOJO_OK) return rc;
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     return DOJO_OK;
   }
   int rc = ensure_staging(h);
   if (rc != DOJO_OK) return rc;
+  const size_t ntr = trace ? (size_t)5 * std::max(0, make_options(opts).max_iter) * B : 0;
+  if (trace && std::max<size_t>(ntr, 1) > h->trace_doubles) {  // grow-only device buffer of the trace (never null: max_iter may be 0)
+    cudaFree(h->d_trace);
+    h->d_trace = nullptr; h->trace_doubles = 0;
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_trace, std::max<size_t>(ntr, 1) * sizeof(double)));
+    h->trace_doubles = std::max<size_t>(ntr, 1);
+  }
   cudaStream_t s = h->stream;
   // inputs: pageable buffers are staged through the handle's pinned buffer, pinned ones are copied from directly
   auto h2d = [&](double* dst, const double* src, double* stage, size_t n) -> cudaError_t {
@@ -862,8 +910,8 @@ extern "C" int dojo_step(DojoHandle* h, const DojoSolverOptions* opts, int B, co
   CUDA_TRY(h, h2d(h->d_Z, Z, pz, (size_t)B * P.nz));
   if (U && P.nu > 0) CUDA_TRY(h, h2d(h->d_U, U, pu, (size_t)B * P.nu));
   if (Fext) CUDA_TRY(h, h2d(h->d_F, Fext, pf, (size_t)B * 6 * P.Nb));
-  rc = dojo_step_async(h, opts, B, h->d_Z, (U && P.nu > 0) ? h->d_U : nullptr, Fext ? h->d_F : nullptr, h->d_Zn, sol ? h->d_sol : nullptr, h->d_status,
-                       h->d_iters, flags, s);
+  rc = launch(h->d_Z, (U && P.nu > 0) ? h->d_U : nullptr, Fext ? h->d_F : nullptr, h->d_Zn, sol ? h->d_sol : nullptr, h->d_status, h->d_iters,
+              trace ? h->d_trace : nullptr, s);
   if (rc != DOJO_OK) return rc;
   // outputs: one stream synchronisation; pageable destinations receive a host copy out of the pinned staging buffer
   double* po = h->p_out;
@@ -876,12 +924,28 @@ extern "C" int dojo_step(DojoHandle* h, const DojoSolverOptions* opts, int B, co
   if (sol) CUDA_TRY(h, cudaMemcpyAsync(sol_pin ? sol : ps, h->d_sol, (size_t)B * P.nres * sizeof(double), cudaMemcpyDeviceToHost, s));
   if (status) CUDA_TRY(h, cudaMemcpyAsync(st_pin ? status : pst, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   if (iters) CUDA_TRY(h, cudaMemcpyAsync(it_pin ? iters : pit, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (ntr) CUDA_TRY(h, cudaMemcpyAsync(trace, h->d_trace, ntr * sizeof(double), cudaMemcpyDeviceToHost, s));  // a diagnostic: no staging
   CUDA_TRY(h, cudaStreamSynchronize(s));
   if (!zn_pin) std::memcpy(Zn, po, (size_t)B * P.nz * sizeof(double));
   if (sol && !sol_pin) std::memcpy(sol, ps, (size_t)B * P.nres * sizeof(double));
   if (status && !st_pin) std::memcpy(status, pst, B * sizeof(int32_t));
   if (iters && !it_pin) std::memcpy(iters, pit, B * sizeof(int32_t));
   return DOJO_OK;
+}
+
+extern "C" int dojo_step(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* Z, const double* U, const double* Fext, double* Zn,
+                         double* sol, int32_t* status, int32_t* iters, uint32_t flags) {
+  if (!h || B <= 0 || B > h->max_batch || !Z || !Zn) { if (h) h->err = "dojo_step: bad arguments (B must be in 1..max_batch)"; return DOJO_EINVAL; }
+  return step_sync(h, opts, B, Z, U, Fext, Zn, sol, status, iters, nullptr, flags);
+}
+
+extern "C" int dojo_step_trace(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* Z, const double* U, const double* Fext, double* Zn,
+                               double* sol, int32_t* status, int32_t* iters, double* trace, uint32_t flags) {
+  if (!h || B <= 0 || B > h->max_batch || !Z || !Zn || !trace) {
+    if (h) h->err = "dojo_step_trace: bad arguments (B must be in 1..max_batch, trace is required)";
+    return DOJO_EINVAL;
+  }
+  return step_sync(h, opts, B, Z, U, Fext, Zn, sol, status, iters, trace, flags);
 }
 
 // simulate!: T steps with the state resident on the device (simulation/simulate.jl:16-36)
@@ -892,7 +956,7 @@ static int launch_rollout(DojoHandle* h, const DojoSolverOptions* opts, int B, i
   a.Z = dZ0; a.U = dU; a.Fext = nullptr; a.Zn = dZf; a.sol = nullptr; a.sol_raw = nullptr; a.status = dstatus; a.iters = nullptr; a.flags = 0;
   a.Fz = nullptr; a.Fu = nullptr; a.Fc = nullptr; a.T = T; a.traj = dtraj; a.done_count = nullptr; a.done_list = nullptr;
   a.counter = h->d_counter; a.prof = h->d_prof; a.order = nullptr; a.prev_iters = nullptr;
-  a.n_peers = 0; a.gather_off = 0;
+  a.n_peers = 0; a.gather_off = 0; a.trace = nullptr;
   enter_call(h, s);
   CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
   a.slot_stride = (int)(h->arena_bytes / sizeof(double));
@@ -1005,7 +1069,7 @@ static int step_grad_impl(DojoHandle* h, const DojoSolverOptions* opts, int B, c
   a.plan = h->plan; a.opts = make_options(opts); a.B = B;
   a.Z = dZ; a.U = dU; a.Fext = dFext; a.Zn = dZn; a.sol = nullptr; a.sol_raw = h->d_gsol; a.status = st; a.iters = nullptr; a.flags = flags;
   a.Fz = dFz; a.Fu = dFu; a.Fc = dFc; a.T = 1; a.traj = nullptr; a.done_count = nullptr; a.done_list = done_list;
-  a.n_peers = 0; a.gather_off = 0;
+  a.n_peers = 0; a.gather_off = 0; a.trace = nullptr;
   a.counter = overlap ? h->d_done + 1 : h->d_counter; a.order = nullptr; a.prev_iters = nullptr;
   a.prof = h->d_prof;
   if (!overlap) CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));

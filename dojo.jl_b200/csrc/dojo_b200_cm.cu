@@ -20,3 +20,7 @@
 extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_kernel(int grad) {
   return grad ? (const void*)dj_cm::dojo_step_kernel<true> : (const void*)dj_cm::dojo_step_kernel<false>;
 }
+// the traced forward kernel of this compilation (dojo_step_trace)
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_trace_kernel() {
+  return (const void*)dj_cm::dojo_step_kernel<false, false, true>;
+}

@@ -1598,8 +1598,18 @@ DJ_DEV void correction(Ctx& c) {
 
 // ------------------------------------------------------------------------------------------------------------
 // mehrotra! (solver/mehrotra.jl:9-73).  Returns the status code; *iters = Newton iterations taken.
+// TRACE (the traced step, dojo_step_trace): the slot's thread 0 also writes one row of 5 doubles per loop-head test into
+// trace[r * 5 + k], row r = head of iteration r + 1, the heads solver_status prints in verbose mode (solver/mehrotra.jl:26-31,
+// 75-98): [rvio, bvio, alpha, mutarget, trials], where alpha (the corrected direction's cone-line-search step), mutarget and
+// trials (line-search trials evaluated up to and including the accepted one) belong to the iteration before the head; row 0 is
+// [rvio, bvio, 1, 0, 0].  Rows after the last head reached are NaN.  TRACE = false compiles to the untraced loop.
 // ------------------------------------------------------------------------------------------------------------
-DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters) {
+DJ_DEV void trace_row(double* tr, int r, double rvio, double bvio, double alpha, double mu, int trials) {
+  double* p = tr + (size_t)r * 5;
+  p[0] = rvio; p[1] = bvio; p[2] = alpha; p[3] = mu; p[4] = (double)trials;
+}
+template <bool TRACE = false>
+DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters, double* trace = nullptr) {
   const Plan& P = *c.P;
   double* A = c.A;
   int status = 1;
@@ -1617,6 +1627,8 @@ DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters) {
   double fk = 0.0, fsel = 0.0;
   int ls_k = 0;
   bool first = true;
+  double alpha_tr = 1.0;  // TRACE: alpha of the current iteration (fk is halved by the line search)
+  int rows_tr = 0;        // TRACE: rows written
   for (;;) {
     double rv, bv, rv2 = 0.0, bv2 = 0.0;
     bool pair = false;
@@ -1695,12 +1707,14 @@ DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters) {
       // decide here, before set_entries! -- the KKT blocks of a final iterate are never used (the gradient pass assembles its own).
       if ((rvio != rvio) || (bvio != bvio)) { status = 3; break; }
       if (ndone >= o.max_iter) break;
+      if (TRACE && c.tid == 0) { trace_row(trace, ndone, rvio, bvio, alpha_tr, mutarget, ls_k + 1); rows_tr = ndone + 1; }
       if ((rvio < o.rtol) && (bvio < o.btol)) { status = 0; break; }
       mode = 0; fk = 0.0;
       continue;  // set_entries! at the new iterate (mu = mutarget)
     }
     // mode 0: the system is assembled
     if (first) { rvio = rv; bvio = bv; first = false; }
+    if (TRACE && c.tid == 0 && rows_tr == 0 && o.max_iter > 0) { trace_row(trace, 0, rvio, bvio, 1.0, 0.0, 0); rows_tr = 1; }  // the first head
     if ((rvio != rvio) || (bvio != bvio)) { status = 3; assist_release(c); break; }
     // `for n = 1:max_iter` tests convergence at the TOP of an iteration only (solver/mehrotra.jl:26-30): an iterate that meets the
     // tolerances after the last iteration's line search is still :failed
@@ -1738,7 +1752,10 @@ DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters) {
       }
     }
     mode = 1; fk = alpha; ls_k = 0;
+    if (TRACE) alpha_tr = alpha;
   }
+  if (TRACE && c.tid == 0)  // NaN padding of the rows after the last head reached
+    for (int k = rows_tr * 5; k < o.max_iter * 5; ++k) trace[k] = nan("");
   *iters = ndone;
   return status;
 }

@@ -50,6 +50,9 @@ struct StepArgs {
   long long gather_off;
   double* peer_buf[DOJO_MAX_GATHER_RANKS];
   unsigned long long* peer_flag[DOJO_MAX_GATHER_RANKS];
+  // traced step (TRACE kernels only, T = 1): [5 x max_iter x B], the rows of mehrotra<true> per environment (dojo_kernels.cuh).  Last
+  // member, so that the parameter offsets of every other member, and with them the untraced kernels, do not depend on it.
+  double* trace;
 };
 
 // epilogue: update_state! + get_next_state (bodies/set.jl:22-36, mechanism/get.jl:126-134).  The default output is the
@@ -85,7 +88,9 @@ __device__ __forceinline__ unsigned long long k_t0g(unsigned long long* prof) { 
 // PLAN_SMEM: the launch keeps its copy of the plan tables in shared memory (a.plan_smem_off >= 0), known at compile time, so that
 // every table pointer is derived from the shared-memory array and the table reads compile to LDS with immediate offsets instead of
 // generic loads (the generic variant, PLAN_SMEM = false, decides at run time and serves mechanisms whose tables do not fit).
-template <bool GRAD, bool PLAN_SMEM = false>
+// TRACE (forward only): the traced step of dojo_step_trace, which also records the solver's loop heads into a.trace.  A compile-time
+// parameter, so that the untraced instantiations are the same code as without it.
+template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false>
 __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(const StepArgs a) {
   extern __shared__ double arena[];
   __shared__ __align__(8) int s_env[128];  // CTA-wide mailbox, layout: dojo_kernels.cuh (cta_align)
@@ -186,7 +191,7 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
         const double* u = a.U ? a.U + ((size_t)t * a.B + e) * P.nu : nullptr;
         const double* fx = a.Fext ? a.Fext + (size_t)e * 6 * P.Nb : nullptr;
         prologue(c, z, u, fx, false);
-        status = mehrotra(c, a.opts, &iters);
+        status = mehrotra<TRACE>(c, a.opts, &iters, TRACE ? a.trace + (size_t)e * max(a.opts.max_iter, 0) * 5 : nullptr);
         worst = max(worst, status);
         // state after this step: the trajectory slot if recorded, else the output buffer (re-read by the next step from L2)
         double* zo = (a.traj ? a.traj + ((size_t)t * a.B + e) * P.nz : a.Zn + (size_t)e * P.nz);

@@ -28,7 +28,7 @@ EXPORTS = ["dojo_default_options", "dojo_create", "dojo_destroy", "dojo_last_err
            "dojo_env_step_async", "dojo_env_reset", "dojo_env_rollout", "dojo_env_policy_rollout", "dojo_update_params", "dojo_num_contact_data", "dojo_step_grad_contact",
            "dojo_step_grad_contact_async", "dojo_step_record", "dojo_step_record_async", "dojo_simulate_record",
            "dojo_gather_create", "dojo_gather_export", "dojo_gather_connect", "dojo_gather_buffer", "dojo_gather_destroy", "dojo_step_gather_async",
-           "dojo_step_grad_gather_async"]
+           "dojo_step_grad_gather_async", "dojo_step_trace", "dojo_step_trace_async"]
 
 _lib = None
 
@@ -59,6 +59,10 @@ def load_library():
     L.dojo_step.restype = C.c_int
     L.dojo_step_async.argtypes = [vp, op, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp]
     L.dojo_step_async.restype = C.c_int
+    L.dojo_step_trace.argtypes = [vp, op, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32]
+    L.dojo_step_trace.restype = C.c_int
+    L.dojo_step_trace_async.argtypes = [vp, op, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp]
+    L.dojo_step_trace_async.restype = C.c_int
     L.dojo_step_grad.argtypes = [vp, op, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32]
     L.dojo_step_grad.restype = C.c_int
     L.dojo_step_grad_async.argtypes = [vp, op, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, vp]
@@ -207,10 +211,13 @@ class BatchedStepper:
         return int(self.L.dojo_launch_count(self.h))
 
     # ------------------------------------------------------------------ host buffers
-    def step(self, Z, U=None, opts: Optional[capi.DojoSolverOptions] = None, fext=None, flags: int = 0, return_sol: bool = False, out=None):
+    def step(self, Z, U=None, opts: Optional[capi.DojoSolverOptions] = None, fext=None, flags: int = 0, return_sol: bool = False, out=None,
+             trace: bool = False):
         """One step! of every environment.  Host arrays in, host arrays out; page-locked arrays (e.g. views of torch pinned
         tensors) are copied from / to directly, pageable ones go through the library's pinned staging buffers.
-        out = (Z_next, status, iters) reuses caller-provided result arrays."""
+        out = (Z_next, status, iters) reuses caller-provided result arrays.
+        trace=True runs the traced step (dojo_step_trace, same results) and appends trace [B, max_iter, 5] to the returned tuple:
+        one row per loop head of the solver, (rvio, bvio, alpha, mu, trials), NaN after the last head reached (include/dojo_b200.h)."""
         Z = np.ascontiguousarray(np.atleast_2d(Z), dtype=np.float64)
         B = Z.shape[0]
         assert Z.shape[1] == self.nz
@@ -228,6 +235,11 @@ class BatchedStepper:
             iters = np.zeros(B, dtype=np.int32)
         sol = np.empty((B, self.nres)) if return_sol else None
         o = opts if opts is not None else capi.solver_options()
+        if trace:
+            tr = np.empty((B, max(int(o.max_iter), 0), 5))
+            rc = self.L.dojo_step_trace(self.h, C.byref(o), B, _p(Z), _p(U), _p(fext), _p(Zn), _p(sol), _p(status), _p(iters), _p(tr), flags)
+            self._check(rc, "dojo_step_trace")
+            return (Zn, status, iters, sol, tr) if return_sol else (Zn, status, iters, tr)
         rc = self.L.dojo_step(self.h, C.byref(o), B, _p(Z), _p(U), _p(fext), _p(Zn), _p(sol), _p(status), _p(iters), flags)
         self._check(rc, "dojo_step")
         return (Zn, status, iters, sol) if return_sol else (Zn, status, iters)
@@ -465,8 +477,14 @@ class BatchedStepper:
 
     # ------------------------------------------------------------------ device buffers (resident data)
     def step_device(self, dZ: int, dU: Optional[int], dZn: int, B: int, opts=None, dstatus: Optional[int] = None, diters: Optional[int] = None,
-                    dsol: Optional[int] = None, dfext: Optional[int] = None, flags: int = 0, stream: int = 0):
+                    dsol: Optional[int] = None, dfext: Optional[int] = None, flags: int = 0, stream: int = 0, dtrace: Optional[int] = None):
+        """dojo_step_async on device pointers; with dtrace ([B, max_iter, 5] doubles) the traced step, dojo_step_trace_async."""
         o = opts if opts is not None else capi.solver_options()
+        if dtrace is not None:
+            rc = self.L.dojo_step_trace_async(self.h, C.byref(o), int(B), _p(dZ), _p(dU), _p(dfext), _p(dZn), _p(dsol), _p(dstatus), _p(diters),
+                                              _p(dtrace), flags, C.c_void_p(int(stream)))
+            self._check(rc, "dojo_step_trace_async")
+            return
         rc = self.L.dojo_step_async(self.h, C.byref(o), int(B), _p(dZ), _p(dU), _p(dfext), _p(dZn), _p(dsol), _p(dstatus), _p(diters), flags,
                                     C.c_void_p(int(stream)))
         self._check(rc, "dojo_step_async")

@@ -187,6 +187,28 @@ int dojo_step_async(DojoHandle* h, const DojoSolverOptions* opts, int B, const d
                     const double* dU, const double* dFext, double* dZ_next, double* dsol,
                     int32_t* dstatus, int32_t* diters, uint32_t flags, void* cuda_stream);
 
+/* Traced step!: dojo_step, and the per-iteration record of the interior-point solver that the reference prints with
+ * SolverOptions(verbose = true) (src/solver/mehrotra.jl:26-31, 75-98).  Every other argument means what it means for
+ * dojo_step / dojo_step_async, and the outputs are bit-identical to theirs.  trace is required: [5 x max_iter x B],
+ * environment e's row r at trace[(e * max_iter + r) * 5 + k].  Row r describes the loop head of Newton iteration r + 1:
+ *   k = 0  rvio    residual violation tested at this head
+ *   k = 1  bvio    bilinear violation tested at this head
+ *   k = 2  alpha   the corrected direction's cone-line-search step of the previous iteration (1 in row 0)
+ *   k = 3  mu      mutarget of the previous iteration (0 in row 0)
+ *   k = 4  trials  line-search trials the previous iteration evaluated up to and including the accepted one (0 in row 0);
+ *                  the step taken was alpha / 2^(trials - 1)
+ * (alpha and mu at a head belong to the iteration before it, as in the reference's printout).  Rows written: n when the
+ * solve converged at head n (iters = n - 1), max_iter when it ended :failed, the heads actually reached when it ended
+ * non-finite; the remaining rows are NaN.  The traced kernel is a separate compilation of the same solver loop: the
+ * untraced entry points do not pay for it. */
+int dojo_step_trace(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* Z, const double* U,
+                    const double* Fext, double* Z_next, double* sol, int32_t* status, int32_t* iters,
+                    double* trace, uint32_t flags);
+int dojo_step_trace_async(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ,
+                          const double* dU, const double* dFext, double* dZ_next, double* dsol,
+                          int32_t* dstatus, int32_t* diters, double* dtrace, uint32_t flags,
+                          void* cuda_stream);
+
 /* step! + consistent IFT gradients at the solution (SURVEY Q2: get_maximal_gradients evaluated
  * right after mehrotra!, before update_state!).  dFz [12Nb x 12Nb x B], dFu [12Nb x nu x B].
  * Two launches on the stream: the forward kernel, then the gradient kernel, which starts on the SMs the
