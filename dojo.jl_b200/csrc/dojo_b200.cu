@@ -26,9 +26,13 @@ using namespace dj;
 // dojo_step_kernel<GRAD> (StepArgs): dojo_step_kernel.cuh; the DJ_ANY_CONTACT compilation of the same source lives in
 // dojo_b200_cm.cu and is reached through these two entry points
 extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_kernel(int grad);
-static const void* step_kernel_fn(bool any_contact, bool grad, bool plan_smem) {
+// small: the forward kernel may be the one specialised for small mechanisms (small_step_ok)
+static const void* step_kernel_fn(bool any_contact, bool grad, bool plan_smem, bool small = false) {
   if (any_contact) return dojo_cm_step_kernel(grad ? 1 : 0);
-  if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return grad ? (const void*)dojo_step_kernel<true, true> : (const void*)dojo_step_kernel<false, true>;
+  if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) {
+    if (!grad && small) return (const void*)dojo_step_kernel<false, true, false, true>;
+    return grad ? (const void*)dojo_step_kernel<true, true> : (const void*)dojo_step_kernel<false, true>;
+  }
   return grad ? (const void*)dojo_step_kernel<true, false> : (const void*)dojo_step_kernel<false, false>;
 }
 // the traced forward kernel (dojo_step_trace) of the compilation and plan placement step_kernel_fn picks for the untraced one
@@ -183,8 +187,19 @@ struct DojoHandle {
   const void* k_fwd_trace = nullptr;               // its traced variant, set up by the first dojo_step_trace call
   double* d_trace = nullptr;                       // grow-only device buffer of dojo_step_trace (host-pointer calls)
   size_t trace_doubles = 0;
+  bool small_step = false;                         // k_fwd is dojo_step_kernel<false, true, false, SMALL = true>
   std::string err;
 };
+// Whether the forward kernel specialised for small mechanisms (dojo_step_kernel.cuh, SMALL) computes this handle's step exactly: the
+// NonlinearContact-only compilation, 2 warps per environment, paired line-search trials and joint pairs, and at most 16 nodes in every
+// role pass (at 2 warps the passes are the bodies, the contacts and the joints, all of a kind), with the whole plan in shared memory
+// (plan_smem_mask: the tables dojo_create places there) read through the shared-memory array (not DOJO_B200_GENERIC_PLAN).
+// DOJO_B200_GENERIC_STEP keeps the generic kernel (A/B measurements).
+static bool small_step_ok(const DojoHandle* h, int plan_smem_mask) {
+  const Plan& P = h->plan;
+  return !h->any_contact && h->nw == 2 && P.nw == 2 && P.jpair && P.ls_pair && std::max(P.Nb, std::max(P.Ne, P.Ni)) <= 16 && plan_smem_mask == 0xff &&
+         !getenv("DOJO_B200_GENERIC_PLAN") && !getenv("DOJO_B200_GENERIC_STEP");
+}
 // [hostemu:handle:end]
 
 static std::string g_create_error;
@@ -667,7 +682,8 @@ extern "C" int dojo_create(const DojoMechanismDesc* d, int device, int max_batch
   };
   plan_prefix(h->slots, h->arena_bytes, &h->plan_smem_off, &h->plan_smem_bytes, &h->plan_smem_mask);
   h->smem_fwd = h->slots * h->arena_bytes + h->plan_smem_bytes;
-  h->k_fwd = step_kernel_fn(h->any_contact, false, h->plan_smem_mask == 0xff);
+  h->small_step = small_step_ok(h, h->plan_smem_mask);
+  h->k_fwd = step_kernel_fn(h->any_contact, false, h->plan_smem_mask == 0xff, h->small_step);
   h->k_grad = step_kernel_fn(h->any_contact, true, false);  // re-selected below once the gradient configuration is known
   // The attribute belongs to the kernel FUNCTION (per device), not to this handle: several handles (ant, pendulum, ...) share the
   // four kernel symbols, so it is set to the device's opt-in maximum once and for all -- a handle created later with a smaller
@@ -728,13 +744,14 @@ extern "C" int64_t dojo_launch_count(const DojoHandle* h) { return h->launches; 
 // debugging aid (DJ_PROFILE builds): cycle counters accumulated by thread 0 of every CTA; out[5]
 // launch configuration chosen by dojo_create (diagnostics: tools/prof_one.py prints it): [slots, slots_grad, gradient chunk width,
 // arena bytes, gradient arena bytes, dynamic smem forward, dynamic smem gradient, plan-in-smem mask forward, mask gradient, paired
-// line-search trials, elimination phases, elimination steps, plan blob bytes, warps per environment, resident CTAs / SM fwd, grad]
+// line-search trials, elimination phases, elimination steps, plan blob bytes, warps per environment, resident CTAs / SM fwd, grad,
+// forward kernel specialised for small mechanisms]
 extern "C" int dojo_debug_config(const DojoHandle* h, int* out) {
   if (!h || !out) return DOJO_EINVAL;
-  const int v[16] = {h->slots, h->slots_grad, h->plan.ch, (int)h->arena_bytes, (int)h->grad_bytes, (int)h->smem_fwd, (int)h->smem_grad,
+  const int v[17] = {h->slots, h->slots_grad, h->plan.ch, (int)h->arena_bytes, (int)h->grad_bytes, (int)h->smem_fwd, (int)h->smem_grad,
                      h->plan_smem_mask, h->plan_smem_mask_grad, h->plan.ls_pair, h->plan.nphase, h->nsteps, h->blob_bytes, h->nw, h->envs_per_sm,
-                     h->envs_per_sm_grad};
-  for (int i = 0; i < 16; ++i) out[i] = v[i];
+                     h->envs_per_sm_grad, h->small_step ? 1 : 0};
+  for (int i = 0; i < 17; ++i) out[i] = v[i];
   return DOJO_OK;
 }
 extern "C" int dojo_debug_cycles(DojoHandle* h, unsigned long long* out) {

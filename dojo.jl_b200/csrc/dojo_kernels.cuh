@@ -135,37 +135,47 @@ DJ_DEV void assist_release(Ctx& c) {
   c.assist = 0;
 }
 
+// SMALL (dojo_step_kernel.cuh): the forward kernel specialised for mechanisms with 2 warps per environment, paired line-search trials
+// and joint pairs, at most 16 nodes in every role pass and the whole plan in shared memory.  Every function below that takes it
+// decides the same things from constants that the generic code reads from the plan; the floating-point operations and their order
+// are the same.  Warps per environment:
+template <bool SMALL>
+DJ_DEV int slot_warps(const Ctx& c) { return SMALL ? 2 : c.P->nw; }
+
 // slot-wide reductions (deterministic: per-warp shuffles, then a fixed-order combine of the nw partials)
+template <bool SMALL = false>
 DJ_DEV void block_nanmax2(const Ctx& c, double& a, double& b) {
   double* red = c.A + c.P->red_off;
   a = warp_nanmax(a);
   b = warp_nanmax(b);
-  if (c.P->nw == 1) return;
+  if (slot_warps<SMALL>(c) == 1) return;
   if (c.lane == 0) { red[2 * c.warp] = a; red[2 * c.warp + 1] = b; }
   slot_sync(c);
   a = red[0]; b = red[1];
-  for (int w = 1; w < c.P->nw; ++w) { a = nanmax(a, red[2 * w]); b = nanmax(b, red[2 * w + 1]); }
+  for (int w = 1; w < slot_warps<SMALL>(c); ++w) { a = nanmax(a, red[2 * w]); b = nanmax(b, red[2 * w + 1]); }
   slot_sync(c);
 }
+template <bool SMALL = false>
 DJ_DEV double block_min(const Ctx& c, double a) {
   double* red = c.A + c.P->red_off;
   a = warp_min(a);
-  if (c.P->nw == 1) return a;
+  if (slot_warps<SMALL>(c) == 1) return a;
   if (c.lane == 0) red[c.warp] = a;
   slot_sync(c);
   a = red[0];
-  for (int w = 1; w < c.P->nw; ++w) a = fmin(a, red[w]);
+  for (int w = 1; w < slot_warps<SMALL>(c); ++w) a = fmin(a, red[w]);
   slot_sync(c);
   return a;
 }
+template <bool SMALL = false>
 DJ_DEV void block_sum3(const Ctx& c, double& a, double& b, double& d) {
   double* red = c.A + c.P->red_off;
   a = warp_sum(a); b = warp_sum(b); d = warp_sum(d);
-  if (c.P->nw == 1) return;
+  if (slot_warps<SMALL>(c) == 1) return;
   if (c.lane == 0) { red[3 * c.warp] = a; red[3 * c.warp + 1] = b; red[3 * c.warp + 2] = d; }
   slot_sync(c);
   a = red[0]; b = red[1]; d = red[2];
-  for (int w = 1; w < c.P->nw; ++w) { a += red[3 * w]; b += red[3 * w + 1]; d += red[3 * w + 2]; }
+  for (int w = 1; w < slot_warps<SMALL>(c); ++w) { a += red[3 * w]; b += red[3 * w + 1]; d += red[3 * w + 2]; }
   slot_sync(c);
 }
 
@@ -1158,7 +1168,8 @@ DJ_DEV void recover_joint(Ctx& c, int idx, double* x) {
   }
 }
 
-template <bool JAC>
+// SMALL: every joint pass takes eval_joint_pair, so that eval_joint<true> is not instantiated.
+template <bool JAC, bool SMALL = false>
 DJ_DEV void evaluate(Ctx& c, double f, int res_off, double& rvio, double& bvio) {
   const Plan& P = *c.P;
   double* A = c.A;
@@ -1170,7 +1181,7 @@ DJ_DEV void evaluate(Ctx& c, double f, int res_off, double& rvio, double& bvio) 
     slot_sync(c);
   }
   for (int p = 0; p < role.npass; ++p) {
-    if (JAC && role.type[p] == ROLE_JOINT && P.jpair && role.count[p] <= 16) {  // set_entries! of the joints on two lanes each (f = 0)
+    if (JAC && role.type[p] == ROLE_JOINT && (SMALL || (P.jpair && role.count[p] <= 16))) {  // set_entries! of the joints on two lanes each (f = 0)
       if ((c.lane >> 1) < role.count[p]) eval_joint_pair(c, role.first[p] + (c.lane >> 1), (c.lane & 1) != 0, res, rv, bv);
       continue;
     }
@@ -1178,7 +1189,7 @@ DJ_DEV void evaluate(Ctx& c, double f, int res_off, double& rvio, double& bvio) 
     if (idx < 0) continue;
     if (role.type[p] == ROLE_BODY) eval_body<JAC>(c, idx, f, res);
     else if (role.type[p] == ROLE_CONTACT) eval_contact<JAC>(c, idx, f, res, rv, bv);
-    else eval_joint<JAC>(c, idx, f, res, rv, bv);
+    else if (!(SMALL && JAC)) eval_joint<JAC>(c, idx, f, res, rv, bv);
   }
 #ifdef DJ_PROFILE
   long long _rw0 = clock64();
@@ -1217,7 +1228,7 @@ DJ_DEV void evaluate(Ctx& c, double f, int res_off, double& rvio, double& bvio) 
 #pragma unroll
     for (int i = 0; i < 6; ++i) rv = nanmax(rv, fabs(rb[i]));
   }
-  block_nanmax2(c, rv, bv);
+  block_nanmax2<SMALL>(c, rv, bv);
   rvio = rv;
   bvio = bv;
   slot_sync(c);
@@ -1232,11 +1243,12 @@ DJ_DEV void evaluate(Ctx& c, double f, int res_off, double& rvio, double& bvio) 
 // `W` is the arena that receives everything this evaluation writes (trial residuals, contribution slots, reduction scratch): the
 // slot's own arena, or -- when a drained slot evaluates trials of another slot's environment (ls_assist_loop) -- the helper's arena
 // while c.A points at the owner's (iterate, direction, per-step constants: read only).
+template <bool SMALL = false>
 DJ_DEV void evaluate_ls(Ctx& c, double* W, double fk, bool pair, double& rvA, double& bvA, double& rvB, double& bvB) {
   const Plan& P = *c.P;
   double* A = c.A;
   const WarpRole& role = c.roles[c.warp];
-  const bool pl = P.ls_pair != 0;
+  const bool pl = SMALL || P.ls_pair != 0;
   const int half = pl ? (c.lane >> 4) : 0;
   const int ln = pl ? (c.lane & 15) : c.lane;
   const bool on = (half == 0) || pair;
@@ -1280,7 +1292,7 @@ DJ_DEV void evaluate_ls(Ctx& c, double* W, double fk, bool pair, double& rvA, do
   if ((c.lane & 15) == 0) { red[4 * c.warp + 2 * (c.lane >> 4)] = rv; red[4 * c.warp + 2 * (c.lane >> 4) + 1] = bv; }
   slot_sync(c);
   rvA = red[0]; bvA = red[1]; rvB = red[2]; bvB = red[3];
-  for (int w = 1; w < P.nw; ++w) {
+  for (int w = 1; w < slot_warps<SMALL>(c); ++w) {
     rvA = nanmax(rvA, red[4 * w]); bvA = nanmax(bvA, red[4 * w + 1]);
     rvB = nanmax(rvB, red[4 * w + 2]); bvB = nanmax(bvB, red[4 * w + 3]);
   }
@@ -1290,6 +1302,7 @@ DJ_DEV void evaluate_ls(Ctx& c, double* W, double fk, bool pair, double& rvA, do
 // ------------------------------------------------------------------------------------------------------------
 // Block LDU (GraphBasedSystems.ldu_factorization! / ldu_backsubstitution!), phase-parallel over the warps
 // ------------------------------------------------------------------------------------------------------------
+template <bool SMALL = false>
 DJ_DEV bool factorize(Ctx& c) {
   const Plan& P = *c.P;
   double* A = c.A;
@@ -1301,7 +1314,7 @@ DJ_DEV bool factorize(Ctx& c) {
   c.f_last = clock64();
 #endif
   for (int ph = 0; ph < P.nphase; ++ph) {
-    const int s0 = c.sched[2 * (ph * P.nw + c.warp)], sn = c.sched[2 * (ph * P.nw + c.warp) + 1];
+    const int s0 = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp)], sn = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp) + 1];
     for (int s = s0 + half; s < s0 + sn; s += 2) {
       const ElimStep& st = c.steps[s];
       double* Dc = A + st.d_off;
@@ -1333,7 +1346,7 @@ DJ_DEV bool factorize(Ctx& c) {
   if (c.lane == 0) flag[c.warp] = wok ? 1 : 0;
   slot_sync(c);
   bool all = true;
-  for (int w = 0; w < P.nw; ++w) all = all && (flag[w] != 0);
+  for (int w = 0; w < slot_warps<SMALL>(c); ++w) all = all && (flag[w] != 0);
   slot_sync(c);
   return all;
 }
@@ -1351,6 +1364,7 @@ DJ_DEV double dot6(const double* a, const double* b, int n) {
 }
 
 // x <- KKT^{-1} x for the vector at arena offset vec_off (solution ordering)
+template <bool SMALL = false>
 DJ_DEV void solve(Ctx& c, int vec_off) {
   const Plan& P = *c.P;
   double* A = c.A;
@@ -1384,7 +1398,7 @@ DJ_DEV void solve(Ctx& c, int vec_off) {
   // intra-step synchronisation is the plain full-warp one: a __syncwarp / shuffle whose member mask DIFFERS between the lanes of one
   // instruction (one 16-lane mask per half) is split into groups with MATCH.ANY by the compiler, whose sequences stall the warp.
   for (int ph = 0; ph < P.nphase; ++ph) {  // forward: z_i -= L~_ic z_c
-    const int s0 = c.sched[2 * (ph * P.nw + c.warp)], sn = c.sched[2 * (ph * P.nw + c.warp) + 1];
+    const int s0 = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp)], sn = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp) + 1];
     for (int it = 0; 2 * it < sn; ++it) {
       const bool act = 2 * it + half < sn;
       const ElimStep& st = c.steps[s0 + 2 * it + (act ? half : 0)];
@@ -1411,7 +1425,7 @@ DJ_DEV void solve(Ctx& c, int vec_off) {
     slot_sync(c);
   }
   for (int ph = P.nphase - 1; ph >= 0; --ph) {  // backward: x_c = D_c^-1 (z_c - sum_j M_cj x_j)
-    const int s0 = c.sched[2 * (ph * P.nw + c.warp)], sn = c.sched[2 * (ph * P.nw + c.warp) + 1];
+    const int s0 = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp)], sn = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp) + 1];
     // same pairing as the forward sweep, last pair first (the steps of one phase are independent)
     for (int it = (sn + 1) / 2 - 1; it >= 0; --it) {
       const bool act = 2 * it + half < sn;
@@ -1464,6 +1478,7 @@ DJ_DEV double soc_step(double l0, double l1, double l2, double d0, double d1, do
   double nr = sqrt(r1 * r1 + r2 * r2);
   return (nr - rs > 0.0) ? fmin(1.0, tau / (nr - rs)) : 1.0;
 }
+template <bool SMALL = false>
 DJ_DEV double cone_line_search(Ctx& c, double tau_ort, double tau_soc) {
   const Plan& P = *c.P;
   const double* sol = c.A + P.sol_off;
@@ -1511,10 +1526,11 @@ DJ_DEV double cone_line_search(Ctx& c, double tau_ort, double tau_soc) {
       for (int i = 0; i < 2 * jd.nb_r; ++i) a = fmin(a, ort_step(sol[jd.sol_off + jd.ne + i], dl[jd.sol_off + jd.ne + i], tau_ort));
     }
   }
-  return block_min(c, a);
+  return block_min<SMALL>(c, a);
 }
 
 // centering! (solver/centering.jl:1-48)
+template <bool SMALL = false>
 DJ_DEV void centering(Ctx& c, double aaff, double& nu, double& nuaff) {
   const Plan& P = *c.P;
   const double* sol = c.A + P.sol_off;
@@ -1555,7 +1571,7 @@ DJ_DEV void centering(Ctx& c, double aaff, double& nu, double& nuaff) {
       cnt += (double)jd.nb_r;
     }
   }
-  block_sum3(c, sn, sa, cnt);
+  block_sum3<SMALL>(c, sn, sa, cnt);
   nu = sn / cnt;
   nuaff = sa / cnt;
 }
@@ -1608,7 +1624,7 @@ DJ_DEV void trace_row(double* tr, int r, double rvio, double bvio, double alpha,
   double* p = tr + (size_t)r * 5;
   p[0] = rvio; p[1] = bvio; p[2] = alpha; p[3] = mu; p[4] = (double)trials;
 }
-template <bool TRACE = false>
+template <bool TRACE = false, bool SMALL = false>
 DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters, double* trace = nullptr) {
   const Plan& P = *c.P;
   double* A = c.A;
@@ -1645,15 +1661,15 @@ DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters, double* trace = nullpt
         c.assist = (P.ls_assist && ai.n_live == 1 && c.nslots > 1 && o.max_ls <= kMaxAssistTrials) ? 1 : 0;
       }
       DJ_TICK(c, t_align)
-      evaluate<true>(c, 0.0, P.rhs_off, rv, bv);
+      evaluate<true, SMALL>(c, 0.0, P.rhs_off, rv, bv);
     } else {
       // trials are evaluated two at a time (k at fk, k + 1 at fk / 2); the second one is used only if the first is rejected
-      pair = (P.ls_pair != 0) && (ls_k + 1 < o.max_ls);
+      pair = (SMALL || P.ls_pair != 0) && (ls_k + 1 < o.max_ls);
       if (c.assist) {  // post the pass: the helpers take the trials behind this slot's own
         if (c.tid == 0) { c.s_int[24] = 1; c.s_int[25] = ls_k; c.s_dbl[0] = fk; c.s_dbl[1] = c.mu; }
         cta_barrier();
       }
-      evaluate_ls(c, A, fk, pair, rv, bv, rv2, bv2);
+      evaluate_ls<SMALL>(c, A, fk, pair, rv, bv, rv2, bv2);
       if (c.assist) {
         if (c.tid == 0) {
           c.s_dbl[2 + 2 * ls_k] = rv; c.s_dbl[3 + 2 * ls_k] = bv;
@@ -1667,7 +1683,7 @@ DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters, double* trace = nullpt
       // line_search! (solver/line_search.jl:1-34): trial k uses alpha / 2^k, accept unless both violations grow
       if (c.assist) {
         // the pass evaluated the trials ls_k .. ls_k + ntr - 1 (this slot's own and the helpers'): same rule, same order
-        const int per = (P.ls_pair != 0) ? 2 : 1;
+        const int per = (SMALL || P.ls_pair != 0) ? 2 : 1;
         const int ntr = min(per * c.nslots, o.max_ls - ls_k);
         bool accepted = false;
         for (int j = 0; j < ntr; ++j) {
@@ -1724,21 +1740,21 @@ DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters, double* trace = nullpt
     for (int t = c.tid; t < P.nres; t += c.nthreads) A[P.sav_off + t] = A[P.rhs_off + t];  // pull_residual!
     slot_sync(c);
     DJ_TICK(c, t_misc)
-    if (!factorize(c)) { status = 3; assist_release(c); break; }
+    if (!factorize<SMALL>(c)) { status = 3; assist_release(c); break; }
     DJ_TICK(c, t_fact)
     double alpha = 1.0;
     for (int pass = 0; pass < 2; ++pass) {  // pass 0: affine direction (Quirk Q3: rhs carries the previous mutarget); pass 1: corrected
       DJ_TICK(c, t_misc)
-      solve(c, P.rhs_off);
+      solve<SMALL>(c, P.rhs_off);
       DJ_TICK(c, t_solve)
       double mx = fmax(rvio, bvio);
       double tau = (pass == 0) ? 0.95 : fmax(0.95, 1.0 - mx * mx);
       DJ_TICK(c, t_misc)
-      alpha = cone_line_search(c, tau, fmin(tau, 0.95));
+      alpha = cone_line_search<SMALL>(c, tau, fmin(tau, 0.95));
       DJ_TICK(c, t_cone)
       if (pass == 0) {
         double nu, nuaff;
-        centering(c, alpha, nu, nuaff);
+        centering<SMALL>(c, alpha, nu, nuaff);
         double ratio = nuaff / (nu + 1e-20);
         double sig = (ratio != ratio) ? ratio : fmin(fmax(ratio, 0.0), 1.0);
         sig = sig * sig * sig;
@@ -1766,10 +1782,11 @@ DJ_DEV int mehrotra(Ctx& c, const Options& o, int* iters, double* trace = nullpt
 // the owner would apply (exact: powers of two), reading the owner's arena and writing residuals, contribution slots and reduction
 // scratch into its own (evaluate_ls, `W`).  The residual evaluations are the ones the owner would have run in later passes, so the
 // accepted trial and its violations -- all the line search hands on -- are bit-identical with and without helpers.
+template <bool SMALL = false>
 DJ_DEV void ls_assist_loop(Ctx& c, const Options& o, int owner, int rank) {
   const Plan& P = *c.P;
   double* own = c.A;
-  const int per = (P.ls_pair != 0) ? 2 : 1;
+  const int per = (SMALL || P.ls_pair != 0) ? 2 : 1;
   for (;;) {
     cta_barrier();  // a pass has been posted, or the iteration released
     if (c.s_int[24] == 0) break;
@@ -1781,7 +1798,7 @@ DJ_DEV void ls_assist_loop(Ctx& c, const Options& o, int owner, int rank) {
       const bool pair = (per == 2) && (k0 + 1 < o.max_ls);
       double rv, bv, rv2, bv2;
       c.A = c.arena0 + (size_t)owner * c.slot_stride;
-      evaluate_ls(c, own, f, pair, rv, bv, rv2, bv2);
+      evaluate_ls<SMALL>(c, own, f, pair, rv, bv, rv2, bv2);
       c.A = own;
       if (c.tid == 0) {
         c.s_dbl[2 + 2 * k0] = rv; c.s_dbl[3 + 2 * k0] = bv;

@@ -90,12 +90,18 @@ __device__ __forceinline__ unsigned long long k_t0g(unsigned long long* prof) { 
 // generic loads (the generic variant, PLAN_SMEM = false, decides at run time and serves mechanisms whose tables do not fit).
 // TRACE (forward only): the traced step of dojo_step_trace, which also records the solver's loop heads into a.trace.  A compile-time
 // parameter, so that the untraced instantiations are the same code as without it.
-template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false>
+// SMALL (forward, PLAN_SMEM, untraced): the launch guarantees nw = 2, Plan::jpair and Plan::ls_pair, at most 16 nodes in every role
+// pass and the whole plan in shared memory (dojo_create: small_step_ok).  The Newton loop then decides from constants what the generic
+// kernel reads from the plan -- the warp count in the reductions, the elimination schedule and the assist arithmetic, the paired
+// line-search branch, the joint pair -- and the one-lane joint assembly eval_joint<true> is not compiled in.  Same floating-point
+// operations in the same order as the generic kernel.
+template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false, bool SMALL = false>
 __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(const StepArgs a) {
+  static_assert(!SMALL || (!GRAD && PLAN_SMEM && !TRACE), "SMALL is a specialisation of the untraced forward kernel with the plan in shared memory");
   extern __shared__ double arena[];
   __shared__ __align__(8) int s_env[128];  // CTA-wide mailbox, layout: dojo_kernels.cuh (cta_align)
   // a CTA hosts a.slots environments at a time; slot k is served by threads [k * 32 nw, (k + 1) * 32 nw)
-  const int slot_threads = 32 * a.plan.nw;
+  const int slot_threads = 32 * (SMALL ? 2 : a.plan.nw);
   const int slot = threadIdx.x / slot_threads;
   Ctx c;
   c.A = arena + (size_t)slot * a.slot_stride;
@@ -191,7 +197,7 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
         const double* u = a.U ? a.U + ((size_t)t * a.B + e) * P.nu : nullptr;
         const double* fx = a.Fext ? a.Fext + (size_t)e * 6 * P.Nb : nullptr;
         prologue(c, z, u, fx, false);
-        status = mehrotra<TRACE>(c, a.opts, &iters, TRACE ? a.trace + (size_t)e * max(a.opts.max_iter, 0) * 5 : nullptr);
+        status = mehrotra<TRACE, SMALL>(c, a.opts, &iters, TRACE ? a.trace + (size_t)e * max(a.opts.max_iter, 0) * 5 : nullptr);
         worst = max(worst, status);
         // state after this step: the trajectory slot if recorded, else the output buffer (re-read by the next step from L2)
         double* zo = (a.traj ? a.traj + ((size_t)t * a.B + e) * P.nz : a.Zn + (size_t)e * P.nz);
@@ -281,7 +287,7 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
     const AlignInfo ai = cta_align(c, false);
     if (ai.n_live == 0) break;
     // one environment left in this CTA: help its line search (same condition as the owner evaluates in mehrotra())
-    if (!GRAD && P.ls_assist && ai.n_live == 1 && a.opts.max_ls <= kMaxAssistTrials) ls_assist_loop(c, a.opts, ai.owner, slot < ai.owner ? slot + 1 : slot);
+    if (!GRAD && P.ls_assist && ai.n_live == 1 && a.opts.max_ls <= kMaxAssistTrials) ls_assist_loop<SMALL>(c, a.opts, ai.owner, slot < ai.owner ? slot + 1 : slot);
   }
   if (!GRAD && a.n_peers > 0) {
     // every environment of this CTA has been written to the peers: make the writes visible system-wide, then count this CTA in on

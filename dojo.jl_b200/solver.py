@@ -199,11 +199,11 @@ class BatchedStepper:
     @property
     def launch_config(self) -> dict:
         """Launch configuration chosen by dojo_create (diagnostics; dojo_debug_config is not part of the public header)."""
-        out = (C.c_int * 16)()
+        out = (C.c_int * 17)()
         self.L.dojo_debug_config.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
         self.L.dojo_debug_config(self.h, out)
         keys = ("slots", "slots_grad", "grad_chunk", "arena_bytes", "grad_arena_bytes", "smem_fwd", "smem_grad", "plan_smem_mask", "plan_smem_mask_grad",
-                "ls_pair", "phases", "steps", "plan_blob_bytes", "warps_per_env", "ctas_per_sm", "ctas_per_sm_grad")
+                "ls_pair", "phases", "steps", "plan_blob_bytes", "warps_per_env", "ctas_per_sm", "ctas_per_sm_grad", "small_step")
         return dict(zip(keys, list(out)))
 
     @property
