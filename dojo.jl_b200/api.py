@@ -10,6 +10,8 @@ Python has no `!`, so `step!` is `step`):
     get_maximal_gradients!(mechanism, z, u; opts)                   get_maximal_gradients(mechanism, z, u, opts=None)
                                           gradients/state.jl:69
     get_contact_gradients(mechanism)      gradients/contact.jl:1    get_contact_gradients(mechanism, z, u, opts=None)
+    simulate! + get_maximal_gradients! at every step                get_trajectory_gradients(mechanism, z0, U, opts=None)
+    simulate! + get_minimal_gradients! at every step                get_minimal_trajectory_gradients(mechanism, x0, U, opts=None)
     mehrotra!(mechanism; opts) -> :success / :failed                status codes returned next to the states (STATUS)
     minimal_to_maximal(mechanism, x)      mechanism/state.jl:9      minimal_to_maximal(mechanism, x)
     maximal_to_minimal(mechanism, z)      mechanism/state.jl:44     maximal_to_minimal(mechanism, z)
@@ -197,6 +199,38 @@ def get_contact_gradients(mechanism: Mechanism, z, u, opts=None, device: int = 0
         _check_single(status)
         return Fz[0], Fc[0]
     return Fz, Fc
+
+
+def _trajectory_inputs(x0, U):
+    x0 = np.asarray(x0, dtype=float)
+    single = x0.ndim == 1
+    X0 = np.atleast_2d(x0)
+    U = np.asarray(U, dtype=float)
+    if single:
+        U = U.reshape(U.shape[0], 1, -1)
+    return single, X0, np.ascontiguousarray(U), U.shape[0]
+
+
+def get_trajectory_gradients(mechanism: Mechanism, z0, U, opts=None, device: int = 0):
+    """simulate!(mechanism, T, ...) from z0 with the open-loop inputs U and get_maximal_gradients! at every step, fused on the device:
+    z0 [13Nb], U [T, nu] -> (Z_traj [T+1, 13Nb] with Z_traj[0] = z0, Fz [T, 12Nb, 12Nb] = dz_{t+1}/dz_t, Fu [T, 12Nb, nu] = dz_{t+1}/du_t,
+    status [T] of every step).  Batched: z0 [B, 13Nb], U [T, B, nu] -> [T+1, B, ...], [T, B, ...], status [T, B]."""
+    single, Z0, U, T = _trajectory_inputs(z0, U)
+    traj, Fz, Fu, status, _ = _stepper(mechanism, Z0.shape[0], device).rollout_grad(Z0, U, T, opts)
+    if single:
+        return traj[:, 0], Fz[:, 0], Fu[:, 0], status[:, 0]
+    return traj, Fz, Fu, status
+
+
+def get_minimal_trajectory_gradients(mechanism: Mechanism, x0, U, opts=None, device: int = 0):
+    """get_trajectory_gradients in minimal coordinates (get_minimal_gradients! at every step): x0 [2nu], U [T, nu] -> (X_traj [T+1, 2nu],
+    Gx [T, 2nu, 2nu], Gu [T, 2nu, nu], status [T]).  The rollout runs in maximal coordinates from minimal_to_maximal(x0); X_traj is its
+    trajectory mapped to minimal coordinates.  Batched: x0 [B, 2nu], U [T, B, nu]."""
+    single, X0, U, T = _trajectory_inputs(x0, U)
+    Xt, Gx, Gu, status, _ = _stepper(mechanism, X0.shape[0], device).rollout_minimal_gradients(X0, U, T, opts)
+    if single:
+        return Xt[:, 0], Gx[:, 0], Gu[:, 0], status[:, 0]
+    return Xt, Gx, Gu, status
 
 
 def minimal_to_maximal(mechanism: Mechanism, x, device: int = 0):

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -41,6 +42,14 @@ static const void* step_trace_kernel_fn(bool any_contact, bool plan_smem) {
   if (any_contact) return dojo_cm_step_trace_kernel();
   if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<false, true, true>;
   return (const void*)dojo_step_kernel<false, false, true>;
+}
+// the recording rollout kernel (dojo_rollout_grad) of the same compilation and plan placement; generic in the warp count, so that it
+// serves every mechanism (the SMALL kernel computes the same step bit for bit)
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_rec_kernel();
+static const void* step_rec_kernel_fn(bool any_contact, bool plan_smem) {
+  if (any_contact) return dojo_cm_step_rec_kernel();
+  if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<false, true, false, false, true>;
+  return (const void*)dojo_step_kernel<false, false, false, false, true>;
 }
 
 // Order of the work queue.  A per-step launch ends when its slowest environment ends: an environment that stalls (ten line-search
@@ -188,6 +197,17 @@ struct DojoHandle {
   double* d_trace = nullptr;                       // grow-only device buffer of dojo_step_trace (host-pointer calls)
   size_t trace_doubles = 0;
   bool small_step = false;                         // k_fwd is dojo_step_kernel<false, true, false, SMALL = true>
+  const void* k_fwd_rec = nullptr;                 // recording rollout kernel (REC), set up by the first dojo_rollout_grad call
+  int envs_per_sm_rec = 1;
+  // dojo_rollout_grad scratch per (environment, step) pair, grow-only: final solutions [nres x pairs], completion list [2 + pairs]
+  // (as d_done), status and iterations [pairs]; host-pointer calls also stage the trajectory [nz x B x (T + 1)], the inputs and the
+  // minimal trajectory
+  double* d_rsol = nullptr;
+  int* d_rdone = nullptr;
+  int32_t *d_rstatus = nullptr, *d_riters = nullptr;
+  size_t rpairs = 0;
+  double *d_rZ = nullptr, *d_rU = nullptr, *d_rX = nullptr;
+  size_t rZ_bytes = 0, rU_bytes = 0, rX_bytes = 0;
   std::string err;
 };
 // Whether the forward kernel specialised for small mechanisms (dojo_step_kernel.cuh, SMALL) computes this handle's step exactly: the
@@ -730,6 +750,7 @@ extern "C" int dojo_destroy(DojoHandle* h) {
   if (h->stream) cudaStreamDestroy(h->stream);
   if (h->ev_last) cudaEventDestroy(h->ev_last);
   cudaFree(h->d_rollU); cudaFree(h->d_rollTraj);
+  cudaFree(h->d_rsol); cudaFree(h->d_rdone); cudaFree(h->d_rstatus); cudaFree(h->d_riters); cudaFree(h->d_rZ); cudaFree(h->d_rU); cudaFree(h->d_rX);
   delete h;
   return DOJO_OK;
 }
@@ -965,13 +986,16 @@ extern "C" int dojo_step_trace(DojoHandle* h, const DojoSolverOptions* opts, int
   return step_sync(h, opts, B, Z, U, Fext, Zn, sol, status, iters, trace, flags);
 }
 
-// simulate!: T steps with the state resident on the device (simulation/simulate.jl:16-36)
+// simulate!: T steps with the state resident on the device (simulation/simulate.jl:16-36).  With dsol_raw, the recording rollout of
+// dojo_rollout_grad (k_fwd_rec): per-step solutions, status [B x T] and iterations (diters, nullable) at pair t * B + e, each pair
+// published on done_list (nullable), states into dtraj = slab 1 of the trajectory whose slab 0 is dZ0; dZf is not written.
 static int launch_rollout(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZf, double* dtraj,
-                          int32_t* dstatus, cudaStream_t s) {
+                          int32_t* dstatus, cudaStream_t s, int32_t* diters = nullptr, double* dsol_raw = nullptr, int* done_count = nullptr,
+                          int* done_list = nullptr) {
   StepArgs a;
   a.plan = h->plan; a.opts = make_options(opts); a.B = B;
-  a.Z = dZ0; a.U = dU; a.Fext = nullptr; a.Zn = dZf; a.sol = nullptr; a.sol_raw = nullptr; a.status = dstatus; a.iters = nullptr; a.flags = 0;
-  a.Fz = nullptr; a.Fu = nullptr; a.Fc = nullptr; a.T = T; a.traj = dtraj; a.done_count = nullptr; a.done_list = nullptr;
+  a.Z = dZ0; a.U = dU; a.Fext = nullptr; a.Zn = dZf; a.sol = nullptr; a.sol_raw = dsol_raw; a.status = dstatus; a.iters = diters; a.flags = 0;
+  a.Fz = nullptr; a.Fu = nullptr; a.Fc = nullptr; a.T = T; a.traj = dtraj; a.done_count = done_count; a.done_list = done_list;
   a.counter = h->d_counter; a.prof = h->d_prof; a.order = nullptr; a.prev_iters = nullptr;
   a.n_peers = 0; a.gather_off = 0; a.trace = nullptr;
   enter_call(h, s);
@@ -979,8 +1003,9 @@ static int launch_rollout(DojoHandle* h, const DojoSolverOptions* opts, int B, i
   a.slot_stride = (int)(h->arena_bytes / sizeof(double));
   a.plan_blob = h->d_blob; a.plan_bytes = h->blob_bytes; a.plan_smem_off = h->plan_smem_off; a.plan_smem_bytes = h->plan_smem_bytes; a.plan_smem_mask = h->plan_smem_mask;
   for (int k = 0; k < 8; ++k) a.plan_off[k] = h->blob_off[k];
-  int grid = std::min((B + h->slots - 1) / h->slots, h->sm_count * h->envs_per_sm);
-  { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(h->k_fwd, dim3(grid), dim3(32 * h->nw * h->slots), kargs, h->smem_fwd, s)); }
+  const bool rec = dsol_raw != nullptr;
+  int grid = std::min((B + h->slots - 1) / h->slots, h->sm_count * (rec ? h->envs_per_sm_rec : h->envs_per_sm));
+  { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(rec ? h->k_fwd_rec : h->k_fwd, dim3(grid), dim3(32 * h->nw * h->slots), kargs, h->smem_fwd, s)); }
   CUDA_TRY(h, cudaGetLastError());
   h->launches += 1;
   leave_call(h, s);
@@ -1041,6 +1066,8 @@ extern "C" int dojo_rollout(DojoHandle* h, const DojoSolverOptions* opts, int B,
 // (two slots per CTA) made it twice as slow.  dZn must not alias dZ (the gradient kernel re-reads the input state).
 static int step_grad_impl(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ, const double* dU, const double* dFext, double* dZn,
                           double* dFz, double* dFu, double* dFc, int32_t* dstatus, int32_t* diters, uint32_t flags, void* cuda_stream, DojoGather* g = nullptr);
+static int launch_grad(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ, const double* dU, const double* dFext, double* dsol_raw,
+                       int32_t* dstatus, double* dFz, double* dFu, double* dFc, uint32_t flags, int* done_list, int* counter, cudaStream_t s);
 extern "C" int dojo_step_grad_async(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ, const double* dU, const double* dFext,
                                     double* dZn, double* dFz, double* dFu, int32_t* dstatus, int32_t* diters, uint32_t flags, void* cuda_stream) {
   return step_grad_impl(h, opts, B, dZ, dU, dFext, dZn, dFz, dFu, nullptr, dstatus, diters, flags, cuda_stream);
@@ -1082,12 +1109,23 @@ static int step_grad_impl(DojoHandle* h, const DojoSolverOptions* opts, int B, c
   }
   int rc = launch_forward(h, opts, B, dZ, dU, dFext, dZn, nullptr, h->d_gsol, st, diters, flags, s, done_count, done_list, g);
   if (rc != DOJO_OK) return rc;
+  rc = launch_grad(h, opts, B, dZ, dU, dFext, h->d_gsol, st, dFz, dFu, dFc, flags, done_list, overlap ? h->d_done + 1 : nullptr, s);
+  if (rc != DOJO_OK) return rc;
+  leave_call(h, s);
+  return DOJO_OK;
+}
+// The gradient kernel over B (state, input, final solution) triples.  done_list non-null: launched programmatically dependent on the
+// forward launch before it on the stream, consuming done_list in order with `counter` (zeroed by the caller) as its work queue; else
+// the handle's work-queue counter, after the forward launch.
+static int launch_grad(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ, const double* dU, const double* dFext, double* dsol_raw,
+                       int32_t* dstatus, double* dFz, double* dFu, double* dFc, uint32_t flags, int* done_list, int* counter, cudaStream_t s) {
+  const bool overlap = done_list != nullptr;
   StepArgs a;
   a.plan = h->plan; a.opts = make_options(opts); a.B = B;
-  a.Z = dZ; a.U = dU; a.Fext = dFext; a.Zn = dZn; a.sol = nullptr; a.sol_raw = h->d_gsol; a.status = st; a.iters = nullptr; a.flags = flags;
+  a.Z = dZ; a.U = dU; a.Fext = dFext; a.Zn = nullptr; a.sol = nullptr; a.sol_raw = dsol_raw; a.status = dstatus; a.iters = nullptr; a.flags = flags;
   a.Fz = dFz; a.Fu = dFu; a.Fc = dFc; a.T = 1; a.traj = nullptr; a.done_count = nullptr; a.done_list = done_list;
   a.n_peers = 0; a.gather_off = 0; a.trace = nullptr;
-  a.counter = overlap ? h->d_done + 1 : h->d_counter; a.order = nullptr; a.prev_iters = nullptr;
+  a.counter = overlap ? counter : h->d_counter; a.order = nullptr; a.prev_iters = nullptr;
   a.prof = h->d_prof;
   if (!overlap) CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
   a.slot_stride = (int)(h->grad_bytes / sizeof(double));
@@ -1109,7 +1147,6 @@ static int step_grad_impl(DojoHandle* h, const DojoSolverOptions* opts, int B, c
   }
   CUDA_TRY(h, cudaGetLastError());
   h->launches += 1;
-  leave_call(h, s);
   return DOJO_OK;
 }
 
@@ -1203,6 +1240,22 @@ extern "C" int dojo_step_grad_gather_async(DojoHandle* h, DojoGather* g, const D
   return gather_close_step(h, g, dstatus, (cudaStream_t)cuda_stream);
 }
 
+// Two chunk buffers of maximal Jacobians (at most 128 MB each, grad_chunk environments or pairs): the kernels of chunk i + 1 run while
+// the gradients of chunk i travel to the host.
+static int ensure_grad_chunks(DojoHandle* h) {
+  if (h->d_Fz[0]) return DOJO_OK;
+  const size_t ng = 12 * (size_t)h->plan.Nb, fz = ng * ng, fu = ng * h->plan.nu;
+  h->grad_chunk = (int)std::max<size_t>(1, std::min<size_t>(h->max_batch, (size_t(128) << 20) / ((fz + fu) * sizeof(double))));
+  for (int k = 0; k < 2; ++k) {
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_Fz[k], (size_t)h->grad_chunk * fz * sizeof(double)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->d_Fu[k], std::max<size_t>(1, (size_t)h->grad_chunk * fu) * sizeof(double)));
+    CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_kernel[k], cudaEventDisableTiming));
+    CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_copy[k], cudaEventDisableTiming));
+  }
+  CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
+  return DOJO_OK;
+}
+
 // Host- or device-pointer entry.  Host buffers are processed in chunks (the Jacobians are large: (12Nb)^2 doubles per env).
 extern "C" int dojo_step_grad(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* Z, const double* U, const double* Fext, double* Zn,
                               double* Fz, double* Fu, int32_t* status, int32_t* iters, uint32_t flags) {
@@ -1216,18 +1269,9 @@ extern "C" int dojo_step_grad(DojoHandle* h, const DojoSolverOptions* opts, int 
     return DOJO_OK;
   }
   int rc = ensure_staging(h);
+  if (rc == DOJO_OK) rc = ensure_grad_chunks(h);
   if (rc != DOJO_OK) return rc;
   const size_t ng = 12 * (size_t)P.Nb, fz = ng * ng, fu = ng * P.nu;
-  if (!h->d_Fz[0]) {  // two chunk buffers: the kernels of chunk i + 1 run while the gradients of chunk i travel to the host
-    h->grad_chunk = (int)std::max<size_t>(1, std::min<size_t>(h->max_batch, (size_t(128) << 20) / ((fz + fu) * sizeof(double))));
-    for (int k = 0; k < 2; ++k) {
-      CUDA_TRY(h, cudaMalloc((void**)&h->d_Fz[k], (size_t)h->grad_chunk * fz * sizeof(double)));
-      CUDA_TRY(h, cudaMalloc((void**)&h->d_Fu[k], std::max<size_t>(1, (size_t)h->grad_chunk * fu) * sizeof(double)));
-      CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_kernel[k], cudaEventDisableTiming));
-      CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_copy[k], cudaEventDisableTiming));
-    }
-    CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-  }
   cudaStream_t s = h->stream, cs = h->copy_stream;
   // whole-batch inputs first (small), per-chunk kernels, gradient copies on the second stream
   CUDA_TRY(h, cudaMemcpyAsync(h->d_Z, Z, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
@@ -1442,17 +1486,9 @@ extern "C" int dojo_minimal_gradients(DojoHandle* h, const DojoSolverOptions* op
   const Plan& P = h->plan;
   cudaStream_t s = h->stream;
   const bool dev = is_device_ptr(X);
-  const size_t ng = 12 * (size_t)P.Nb, fz = ng * ng, fu = ng * P.nu, nm = 2 * (size_t)P.nu, gx = nm * nm, gu = nm * P.nu;
-  if (!h->d_Fz[0]) {  // same chunk buffers as the host-pointer path of dojo_step_grad
-    h->grad_chunk = (int)std::max<size_t>(1, std::min<size_t>(h->max_batch, (size_t(128) << 20) / ((fz + fu) * sizeof(double))));
-    for (int k = 0; k < 2; ++k) {
-      CUDA_TRY(h, cudaMalloc((void**)&h->d_Fz[k], (size_t)h->grad_chunk * fz * sizeof(double)));
-      CUDA_TRY(h, cudaMalloc((void**)&h->d_Fu[k], std::max<size_t>(1, (size_t)h->grad_chunk * fu) * sizeof(double)));
-      CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_kernel[k], cudaEventDisableTiming));
-      CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_copy[k], cudaEventDisableTiming));
-    }
-    CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-  }
+  const size_t nm = 2 * (size_t)P.nu, gx = nm * nm, gu = nm * P.nu;
+  rc = ensure_grad_chunks(h);  // same chunk buffers as the host-pointer path of dojo_step_grad
+  if (rc != DOJO_OK) return rc;
   const double* dX = X;
   const double* dU = (U && P.nu > 0) ? U : nullptr;
   double *dXn = X_next, *dGx = Gx, *dGu = Gu;
@@ -1484,6 +1520,188 @@ extern "C" int dojo_minimal_gradients(DojoHandle* h, const DojoSolverOptions* op
     if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   }
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  return DOJO_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Trajectory Jacobians: simulate! + get_maximal_gradients! / get_minimal_gradients! at every step (include/dojo_b200.h)
+// ------------------------------------------------------------------------------------------------------------
+// One recording rollout (REC kernel) advances B environments T steps and keeps, per pair p = t * B + e, the final solution, status
+// and iterations; the trajectory [nz x B x (T + 1)] holds Z0 in slab 0, so that [feature x B x T] is [feature x pairs] and the unchanged
+// gradient kernel runs over the pairs with a.Z = slab 0.
+static int ensure_rec_kernel(DojoHandle* h) {
+  if (h->k_fwd_rec) return DOJO_OK;
+  const void* k = step_rec_kernel_fn(h->any_contact, h->plan_smem_mask == 0xff);
+  int optin = 0, occ = 1;
+  cudaFuncAttributes fa;
+  CUDA_TRY(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+  CUDA_TRY(h, cudaFuncGetAttributes(&fa, k));
+  CUDA_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
+  CUDA_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, 32 * h->nw * h->slots, h->smem_fwd));
+  h->envs_per_sm_rec = std::max(1, occ);
+  h->k_fwd_rec = k;
+  return DOJO_OK;
+}
+
+// grow-only device buffer; a buffer that is replaced may still be read by the handle's last call
+static int grow_buffer(DojoHandle* h, void** buf, size_t* have, size_t need) {
+  if (*have >= need) return DOJO_OK;
+  CUDA_TRY(h, cudaDeviceSynchronize());
+  cudaFree(*buf); *buf = nullptr; *have = 0;
+  CUDA_TRY(h, cudaMalloc(buf, need));
+  *have = need;
+  return DOJO_OK;
+}
+
+static int ensure_rollout_grad_scratch(DojoHandle* h, size_t pairs) {
+  if (h->rpairs >= pairs) return DOJO_OK;
+  CUDA_TRY(h, cudaDeviceSynchronize());
+  cudaFree(h->d_rsol); cudaFree(h->d_rdone); cudaFree(h->d_rstatus); cudaFree(h->d_riters);
+  h->d_rsol = nullptr; h->d_rdone = nullptr; h->d_rstatus = nullptr; h->d_riters = nullptr; h->rpairs = 0;
+  CUDA_TRY(h, cudaMalloc((void**)&h->d_rsol, pairs * h->plan.nres * sizeof(double)));
+  CUDA_TRY(h, cudaMalloc((void**)&h->d_rdone, (pairs + 2) * sizeof(int)));
+  CUDA_TRY(h, cudaMalloc((void**)&h->d_rstatus, pairs * sizeof(int32_t)));
+  CUDA_TRY(h, cudaMalloc((void**)&h->d_riters, pairs * sizeof(int32_t)));
+  h->rpairs = pairs;
+  return DOJO_OK;
+}
+
+// argument checks and set-up shared by the three entries: no launch before every check has passed
+static int rollout_grad_setup(DojoHandle* h, int B, int T, bool buffers, const char* who) {
+  if (!h) return DOJO_EINVAL;
+  if (B <= 0 || B > h->max_batch || T <= 0 || !buffers || (long long)B * (T + 1) > (long long)INT_MAX - 2) {
+    h->err = std::string(who) + ": bad arguments (B in 1..max_batch, T >= 1, B * (T + 1) < 2^31 - 2, state / trajectory / Jacobian buffers required)";
+    return DOJO_EINVAL;
+  }
+  if (!h->grad_bytes) { h->err = std::string(who) + ": the gradient workspace does not fit in shared memory for this mechanism"; return DOJO_ENOMEM; }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  int rc = ensure_rec_kernel(h);
+  if (rc == DOJO_OK) rc = ensure_rollout_grad_scratch(h, (size_t)B * T);
+  return rc;
+}
+
+extern "C" int dojo_rollout_grad_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZ_traj,
+                                       double* dFz, double* dFu, int32_t* dstatus, int32_t* diters, void* cuda_stream) {
+  int rc = rollout_grad_setup(h, B, T, dZ0 && dZ_traj && dFz && dFu, "dojo_rollout_grad_async");
+  if (rc != DOJO_OK) return rc;
+  const Plan& P = h->plan;
+  cudaStream_t s = (cudaStream_t)cuda_stream;
+  const int pairs = B * T;
+  int32_t* st = dstatus ? dstatus : h->d_rstatus;
+  enter_call(h, s);
+  if (dZ0 != dZ_traj) CUDA_TRY(h, cudaMemcpyAsync(dZ_traj, dZ0, (size_t)B * P.nz * sizeof(double), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_rdone, 0, 2 * sizeof(int), s));                     // [0] finished pairs, [1] gradient work queue
+  CUDA_TRY(h, cudaMemsetAsync(h->d_rdone + 2, 0xff, (size_t)pairs * sizeof(int), s));  // -1 = not finished yet
+  // the gradients of early steps run on the SMs the rollout's tail leaves idle while later steps are still being solved
+  rc = launch_rollout(h, opts, B, T, dZ_traj, dU, nullptr, dZ_traj + (size_t)B * P.nz, st, s, diters, h->d_rsol, h->d_rdone, h->d_rdone + 2);
+  if (rc == DOJO_OK) rc = launch_grad(h, opts, pairs, dZ_traj, dU, nullptr, h->d_rsol, st, dFz, dFu, nullptr, 0, h->d_rdone + 2, h->d_rdone + 1, s);
+  if (rc != DOJO_OK) return rc;
+  leave_call(h, s);
+  return DOJO_OK;
+}
+
+// Host- or device-pointer entry.  With host buffers the Jacobians (ant: ~212 KB per pair) go to the host in chunks of pairs through the
+// two chunk buffers of dojo_step_grad, after one rollout; the gradient kernel of chunk i + 1 runs while chunk i is being copied.
+extern "C" int dojo_rollout_grad(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const double* U, double* Z_traj,
+                                 double* Fz, double* Fu, int32_t* status, int32_t* iters) {
+  int rc = rollout_grad_setup(h, B, T, Z0 && Z_traj && Fz && Fu, "dojo_rollout_grad");
+  if (rc != DOJO_OK) return rc;
+  if (is_device_ptr(Z0)) {
+    rc = dojo_rollout_grad_async(h, opts, B, T, Z0, U, Z_traj, Fz, Fu, status, iters, h->stream);
+    if (rc != DOJO_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    return DOJO_OK;
+  }
+  rc = ensure_grad_chunks(h);
+  const Plan& P = h->plan;
+  const size_t pairs = (size_t)B * T, ng = 12 * (size_t)P.Nb, fz = ng * ng, fu = ng * P.nu;
+  const bool has_u = U && P.nu > 0;
+  if (rc == DOJO_OK) rc = grow_buffer(h, (void**)&h->d_rZ, &h->rZ_bytes, (pairs + B) * P.nz * sizeof(double));
+  if (rc == DOJO_OK && has_u) rc = grow_buffer(h, (void**)&h->d_rU, &h->rU_bytes, pairs * P.nu * sizeof(double));
+  if (rc != DOJO_OK) return rc;
+  cudaStream_t s = h->stream, cs = h->copy_stream;
+  const double* dU = has_u ? h->d_rU : nullptr;
+  CUDA_TRY(h, cudaMemcpyAsync(h->d_rZ, Z0, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
+  if (has_u) CUDA_TRY(h, cudaMemcpyAsync(h->d_rU, U, pairs * P.nu * sizeof(double), cudaMemcpyHostToDevice, s));
+  rc = launch_rollout(h, opts, B, T, h->d_rZ, dU, nullptr, h->d_rZ + (size_t)B * P.nz, h->d_rstatus, s, h->d_riters, h->d_rsol);
+  if (rc != DOJO_OK) return rc;
+  int k = 0;
+  for (size_t p0 = 0; p0 < pairs; p0 += h->grad_chunk, k ^= 1) {
+    const int n = (int)std::min<size_t>(h->grad_chunk, pairs - p0);
+    if (p0 >= 2 * (size_t)h->grad_chunk) CUDA_TRY(h, cudaStreamWaitEvent(s, h->ev_copy[k], 0));  // buffer k has been drained
+    enter_call(h, s);
+    rc = launch_grad(h, opts, n, h->d_rZ + p0 * P.nz, dU ? dU + p0 * P.nu : nullptr, nullptr, h->d_rsol + p0 * P.nres, h->d_rstatus + p0, h->d_Fz[k],
+                     h->d_Fu[k], nullptr, 0, nullptr, nullptr, s);
+    if (rc != DOJO_OK) return rc;
+    leave_call(h, s);
+    CUDA_TRY(h, cudaEventRecord(h->ev_kernel[k], s));
+    CUDA_TRY(h, cudaStreamWaitEvent(cs, h->ev_kernel[k], 0));
+    CUDA_TRY(h, cudaMemcpyAsync(Fz + p0 * fz, h->d_Fz[k], (size_t)n * fz * sizeof(double), cudaMemcpyDeviceToHost, cs));
+    if (fu) CUDA_TRY(h, cudaMemcpyAsync(Fu + p0 * fu, h->d_Fu[k], (size_t)n * fu * sizeof(double), cudaMemcpyDeviceToHost, cs));
+    CUDA_TRY(h, cudaEventRecord(h->ev_copy[k], cs));
+  }
+  CUDA_TRY(h, cudaMemcpyAsync(Z_traj, h->d_rZ, (pairs + B) * P.nz * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_rstatus, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_riters, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  CUDA_TRY(h, cudaStreamSynchronize(cs));
+  return DOJO_OK;
+}
+
+// The same in minimal coordinates (get_minimal_gradients! at every step): minimal_to_maximal of X0, the recording rollout, then per
+// chunk of pairs the gradient kernel and the map-Jacobian kernel in mode 2 between slabs t and t + 1 (the maximal Jacobians never leave
+// the device), and finally maximal_to_minimal of all T + 1 slabs.  Host or device pointers (all of the same kind).
+extern "C" int dojo_rollout_minimal_gradients(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* X0, const double* U,
+                                              double* X_traj, double* Gx, double* Gu, int32_t* status, int32_t* iters) {
+  int rc = rollout_grad_setup(h, B, T, X0 && X_traj && Gx && Gu, "dojo_rollout_minimal_gradients");
+  if (rc != DOJO_OK) return rc;
+  const Plan& P = h->plan;
+  const size_t pairs = (size_t)B * T, nm = 2 * (size_t)P.nu, gx = nm * nm, gu = nm * P.nu;
+  const bool dev = is_device_ptr(X0), has_u = U && P.nu > 0;
+  rc = ensure_staging(h);
+  if (rc == DOJO_OK) rc = ensure_grad_chunks(h);
+  if (rc == DOJO_OK) rc = grow_buffer(h, (void**)&h->d_rZ, &h->rZ_bytes, (pairs + B) * P.nz * sizeof(double));
+  if (rc == DOJO_OK && !dev && has_u) rc = grow_buffer(h, (void**)&h->d_rU, &h->rU_bytes, pairs * P.nu * sizeof(double));
+  if (rc == DOJO_OK && !dev) rc = grow_buffer(h, (void**)&h->d_rX, &h->rX_bytes, std::max<size_t>(1, (pairs + B) * nm) * sizeof(double));
+  if (rc == DOJO_OK && !dev) rc = ensure_kjout(h, (size_t)h->grad_chunk * (gx + gu));
+  if (rc != DOJO_OK) return rc;
+  cudaStream_t s = h->stream;
+  const double* dX0 = X0;
+  const double* dU = has_u ? U : nullptr;
+  int32_t* dst = (dev && status) ? status : h->d_rstatus;
+  int32_t* dit = (dev && iters) ? iters : h->d_riters;
+  if (!dev) {
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_X, X0, (size_t)B * nm * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (has_u) { CUDA_TRY(h, cudaMemcpyAsync(h->d_rU, U, pairs * P.nu * sizeof(double), cudaMemcpyHostToDevice, s)); dU = h->d_rU; }
+    dX0 = h->d_X;
+  }
+  enter_call(h, s);
+  rc = launch_kin(h, true, B, dX0, h->d_rZ, s);
+  if (rc == DOJO_OK) rc = launch_rollout(h, opts, B, T, h->d_rZ, dU, nullptr, h->d_rZ + (size_t)B * P.nz, dst, s, dit, h->d_rsol);
+  if (rc != DOJO_OK) return rc;
+  for (size_t p0 = 0; p0 < pairs; p0 += h->grad_chunk) {
+    const int n = (int)std::min<size_t>(h->grad_chunk, pairs - p0);
+    double* oGx = dev ? Gx + p0 * gx : h->d_kjout;
+    double* oGu = dev ? Gu + p0 * gu : h->d_kjout + (size_t)n * gx;
+    rc = launch_grad(h, opts, n, h->d_rZ + p0 * P.nz, dU ? dU + p0 * P.nu : nullptr, nullptr, h->d_rsol + p0 * P.nres, dst + p0, h->d_Fz[0], h->d_Fu[0],
+                     nullptr, 0, nullptr, nullptr, s);
+    if (rc == DOJO_OK) rc = launch_kinjac(h, 2, n, h->d_rZ + p0 * P.nz, h->d_rZ + (p0 + B) * P.nz, h->d_Fz[0], h->d_Fu[0], oGx, oGu, s);
+    if (rc != DOJO_OK) return rc;
+    if (!dev) {
+      CUDA_TRY(h, cudaMemcpyAsync(Gx + p0 * gx, oGx, (size_t)n * gx * sizeof(double), cudaMemcpyDeviceToHost, s));
+      if (gu) CUDA_TRY(h, cudaMemcpyAsync(Gu + p0 * gu, oGu, (size_t)n * gu * sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+  }
+  rc = launch_kin(h, false, (int)(pairs + B), h->d_rZ, dev ? X_traj : h->d_rX, s);
+  if (rc != DOJO_OK) return rc;
+  if (!dev) {
+    CUDA_TRY(h, cudaMemcpyAsync(X_traj, h->d_rX, (pairs + B) * nm * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_rstatus, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_riters, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  }
+  leave_call(h, s);
   CUDA_TRY(h, cudaStreamSynchronize(s));
   return DOJO_OK;
 }

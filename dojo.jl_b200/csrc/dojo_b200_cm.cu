@@ -24,3 +24,7 @@ extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_kernel
 extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_trace_kernel() {
   return (const void*)dj_cm::dojo_step_kernel<false, false, true>;
 }
+// the recording rollout kernel of this compilation (dojo_rollout_grad)
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_rec_kernel() {
+  return (const void*)dj_cm::dojo_step_kernel<false, false, false, false, true>;
+}

@@ -95,9 +95,14 @@ __device__ __forceinline__ unsigned long long k_t0g(unsigned long long* prof) { 
 // kernel reads from the plan -- the warp count in the reductions, the elimination schedule and the assist arithmetic, the paired
 // line-search branch, the joint pair -- and the one-lane joint assembly eval_joint<true> is not compiled in.  Same floating-point
 // operations in the same order as the generic kernel.
-template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false, bool SMALL = false>
+// REC (forward, untraced, generic): the recording rollout of dojo_rollout_grad.  After step t of environment e it keeps what the gradient
+// kernel needs at pair p = t * B + e -- the final solution in sol_raw [nres x B x T], status [B x T], iters [B x T] (nullable) -- and
+// publishes p on done_list (nullable).  a.traj is slab 1 of the [nz x B x (T + 1)] trajectory whose slab 0 is a.Z, so that pair p
+// starts from a.Z + p * nz; Zn is not written.  A compile-time parameter, so that the other instantiations are the same code as without it.
+template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false, bool SMALL = false, bool REC = false>
 __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(const StepArgs a) {
   static_assert(!SMALL || (!GRAD && PLAN_SMEM && !TRACE), "SMALL is a specialisation of the untraced forward kernel with the plan in shared memory");
+  static_assert(!REC || (!GRAD && !TRACE && !SMALL), "REC is a variant of the generic untraced forward kernel");
   extern __shared__ double arena[];
   __shared__ __align__(8) int s_env[128];  // CTA-wide mailbox, layout: dojo_kernels.cuh (cta_align)
   // a CTA hosts a.slots environments at a time; slot k is served by threads [k * 32 nw, (k + 1) * 32 nw)
@@ -202,14 +207,31 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
         // state after this step: the trajectory slot if recorded, else the output buffer (re-read by the next step from L2)
         double* zo = (a.traj ? a.traj + ((size_t)t * a.B + e) * P.nz : a.Zn + (size_t)e * P.nz);
         epilogue(c, zo, (a.flags & DOJO_FLAG_Q1_LITERAL_RETURN) != 0, (t + 1 == a.T) ? a.n_peers : 0, a.peer_buf, a.gather_off + (long long)e * P.nz);
+        if (REC) {  // pair t * B + e: its solution, status and iterations, visible before the pair appears in done_list
+          const size_t p = (size_t)t * a.B + e;
+          for (int k = c.tid; k < P.nres; k += c.nthreads) a.sol_raw[p * P.nres + k] = c.A[P.sol_off + k];
+          if (c.tid == 0) {
+            a.status[p] = status;
+            if (a.iters) a.iters[p] = iters;
+          }
+          if (a.done_list) {
+            __threadfence();
+            slot_sync(c);
+            if (c.tid == 0) {
+              const int pos = atomicAdd(a.done_count, 1);
+              __threadfence();
+              ((volatile int*)a.done_list)[pos] = (int)p;
+            }
+          }
+        }
         if (t + 1 < a.T) { __threadfence_block(); slot_sync(c); z = zo; }
       }
-      if (a.traj) {  // final state also goes to Zn
+      if (a.traj && !REC) {  // final state also goes to Zn
         slot_sync(c);
         for (int k = c.tid; k < P.nz; k += c.nthreads) a.Zn[(size_t)e * P.nz + k] = a.traj[((size_t)(a.T - 1) * a.B + e) * P.nz + k];
       }
       status = worst;
-      if (a.sol_raw)
+      if (a.sol_raw && !REC)
         for (int t = c.tid; t < P.nres; t += c.nthreads) a.sol_raw[(size_t)e * P.nres + t] = c.A[P.sol_off + t];
     } else {
       // gradient pass (get_maximal_gradients!, gradients/state.jl:69-126) at the solution the forward launch left in
@@ -263,8 +285,8 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
       }
     }
     if (c.tid == 0) {
-      if (a.status) a.status[e] = status;
-      if (!GRAD) {
+      if (a.status && !REC) a.status[e] = status;
+      if (!GRAD && !REC) {
         if (a.iters) a.iters[e] = iters;
         if (a.prev_iters) a.prev_iters[e] = iters;
       }
@@ -272,7 +294,7 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
       if (a.prof) { unsigned long long e_t1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(e_t1)); a.prof[32 + 2 * e] = e_t0 - k_t0g(a.prof); a.prof[33 + 2 * e] = e_t1 - e_t0; }
 #endif
     }
-    if (!GRAD && a.done_list) {  // publish: results of this environment are visible before its index appears in the list
+    if (!GRAD && !REC && a.done_list) {  // publish: results of this environment are visible before its index appears in the list
       __threadfence();
       slot_sync(c);
       if (c.tid == 0) {

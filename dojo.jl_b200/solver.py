@@ -28,7 +28,8 @@ EXPORTS = ["dojo_default_options", "dojo_create", "dojo_destroy", "dojo_last_err
            "dojo_env_step_async", "dojo_env_reset", "dojo_env_rollout", "dojo_env_policy_rollout", "dojo_update_params", "dojo_num_contact_data", "dojo_step_grad_contact",
            "dojo_step_grad_contact_async", "dojo_step_record", "dojo_step_record_async", "dojo_simulate_record",
            "dojo_gather_create", "dojo_gather_export", "dojo_gather_connect", "dojo_gather_buffer", "dojo_gather_destroy", "dojo_step_gather_async",
-           "dojo_step_grad_gather_async", "dojo_step_trace", "dojo_step_trace_async"]
+           "dojo_step_grad_gather_async", "dojo_step_trace", "dojo_step_trace_async", "dojo_rollout_grad", "dojo_rollout_grad_async",
+           "dojo_rollout_minimal_gradients"]
 
 _lib = None
 
@@ -117,6 +118,12 @@ def load_library():
     L.dojo_step_record_async.restype = C.c_int
     L.dojo_simulate_record.argtypes = [vp, op, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
     L.dojo_simulate_record.restype = C.c_int
+    L.dojo_rollout_grad.argtypes = [vp, op, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_grad.restype = C.c_int
+    L.dojo_rollout_grad_async.argtypes = [vp, op, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_grad_async.restype = C.c_int
+    L.dojo_rollout_minimal_gradients.argtypes = [vp, op, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_minimal_gradients.restype = C.c_int
     L.dojo_gather_create.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
     L.dojo_gather_create.restype = C.c_int
     L.dojo_gather_export.argtypes = [vp, vp]
@@ -295,6 +302,43 @@ class BatchedStepper:
         rc = self.L.dojo_rollout(self.h, C.byref(o), B, int(T), _p(Z0), _p(U), _p(Zf), _p(traj), _p(st))
         self._check(rc, "dojo_rollout")
         return (Zf, st, traj) if record else (Zf, st)
+
+    def rollout_grad(self, Z0, U=None, T: int = 1, opts=None):
+        """T fused steps and the IFT Jacobians of every step (dojo_rollout_grad): simulate! + get_maximal_gradients! at each step.
+        U [T, B, nu] or None.  Returns (Z_traj [T+1, B, 13Nb] with Z_traj[0] = Z0 and Z_traj[t+1] the state after step t,
+        Fz [T, B, 12Nb, 12Nb], Fu [T, B, 12Nb, nu] with Fz[t, e] = dz_{t+1}/dz_t, status [T, B], iters [T, B]); Fz / Fu are transposed
+        views of the column-major per-pair buffers, as in step_grad."""
+        Z0 = np.ascontiguousarray(np.atleast_2d(Z0), dtype=np.float64)
+        B, T, ng = Z0.shape[0], int(T), self.ngrad
+        assert Z0.shape[1] == self.nz
+        if U is not None:
+            U = np.ascontiguousarray(U, dtype=np.float64)
+            assert U.shape == (T, B, self.nu)
+        traj = np.empty((max(T, 0) + 1, B, self.nz))
+        Fz, Fu = np.empty((max(T, 0), B, ng, ng)), np.empty((max(T, 0), B, self.nu, ng))
+        status, iters = np.zeros((max(T, 0), B), dtype=np.int32), np.zeros((max(T, 0), B), dtype=np.int32)
+        o = opts if opts is not None else capi.solver_options()
+        rc = self.L.dojo_rollout_grad(self.h, C.byref(o), B, T, _p(Z0), _p(U), _p(traj), _p(Fz), _p(Fu), _p(status), _p(iters))
+        self._check(rc, "dojo_rollout_grad")
+        return traj, np.transpose(Fz, (0, 1, 3, 2)), np.transpose(Fu, (0, 1, 3, 2)), status, iters
+
+    def rollout_minimal_gradients(self, X0, U=None, T: int = 1, opts=None):
+        """The same in minimal coordinates (dojo_rollout_minimal_gradients): the rollout from minimal_to_maximal(X0) and
+        get_minimal_gradients! at every step.  Returns (X_traj [T+1, B, 2nu], Gx [T, B, 2nu, 2nu], Gu [T, B, 2nu, nu], status [T, B],
+        iters [T, B])."""
+        X0 = np.ascontiguousarray(np.atleast_2d(X0), dtype=np.float64)
+        B, T, nm = X0.shape[0], int(T), self.nmin
+        assert X0.shape[1] == nm
+        if U is not None:
+            U = np.ascontiguousarray(U, dtype=np.float64)
+            assert U.shape == (T, B, self.nu)
+        Xt = np.empty((max(T, 0) + 1, B, nm))
+        Gx, Gu = np.empty((max(T, 0), B, nm, nm)), np.empty((max(T, 0), B, self.nu, nm))
+        status, iters = np.zeros((max(T, 0), B), dtype=np.int32), np.zeros((max(T, 0), B), dtype=np.int32)
+        o = opts if opts is not None else capi.solver_options()
+        rc = self.L.dojo_rollout_minimal_gradients(self.h, C.byref(o), B, T, _p(X0), _p(U), _p(Xt), _p(Gx), _p(Gu), _p(status), _p(iters))
+        self._check(rc, "dojo_rollout_minimal_gradients")
+        return Xt, np.transpose(Gx, (0, 1, 3, 2)), np.transpose(Gu, (0, 1, 3, 2)), status, iters
 
     # ------------------------------------------------------------------ minimal coordinates (SURVEY 8 f1)
     @property
@@ -520,6 +564,15 @@ class BatchedStepper:
         rc = self.L.dojo_step_grad_async(self.h, C.byref(o), int(B), _p(dZ), _p(dU), None, _p(dZn), _p(dFz), _p(dFu), _p(dstatus), _p(diters), flags,
                                          C.c_void_p(int(stream)))
         self._check(rc, "dojo_step_grad_async")
+
+    def rollout_grad_device(self, dZ0: int, dU: Optional[int], dZ_traj: int, dFz: int, dFu: int, B: int, T: int, opts=None, dstatus=None,
+                            diters=None, stream: int = 0):
+        """dojo_rollout_grad_async on device pointers: Z_traj [T+1, B, 13Nb], Fz [T, B, 12Nb, 12Nb] and Fu [T, B, nu, 12Nb] (column-major
+        per pair), status / iters [T, B]; dZ0 may be dZ_traj (slab 0 already holds Z0)."""
+        o = opts if opts is not None else capi.solver_options()
+        rc = self.L.dojo_rollout_grad_async(self.h, C.byref(o), int(B), int(T), _p(dZ0), _p(dU), _p(dZ_traj), _p(dFz), _p(dFu), _p(dstatus),
+                                            _p(diters), C.c_void_p(int(stream)))
+        self._check(rc, "dojo_rollout_grad_async")
 
     # ---- multi-GPU: the exchange of the next states fused into the step (include/dojo_b200.h, SURVEY.md 8e)
     def gather_create(self, world: int, rank: int, B_local: int):

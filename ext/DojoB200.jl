@@ -248,6 +248,28 @@ function rollout(mech::Mechanism, Z0::Matrix{Float64}, U::Array{Float64,3}; opts
     return Zf, traj
 end
 
+"simulate! + get_maximal_gradients! at every step, fused: U is nu x B x T; returns (Z_traj 13Nb x B x (T+1) with Z_traj[:, :, 1] = Z0,
+ Fz 12Nb x 12Nb x B x T, Fu 12Nb x nu x B x T, status B x T) -- Fz[:, :, e, t] = dz_{t+1}/dz_t"
+function rollout_gradients(mech::Mechanism, Z0::Matrix{Float64}, U::Array{Float64,3}; opts = SolverOptions{Float64}())
+    h = handle(mech); B = size(Z0, 2); T = size(U, 3); ng = 12 * length(mech.bodies)
+    traj = zeros(h.nz, B, T + 1); Fz = zeros(ng, ng, B, T); Fu = zeros(ng, h.nu, B, T); status = zeros(Int32, B, T); iters = zeros(Int32, B, T)
+    rc = ccall((:dojo_rollout_grad, LIB), Cint,
+               (Ptr{Cvoid}, Ref{COptions}, Cint, Cint, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}, Ptr{Int32}),
+               h.ptr, COptions(opts), B, T, Z0, U, traj, Fz, Fu, status, iters)
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return traj, Fz, Fu, status
+end
+"the same in minimal coordinates (get_minimal_gradients! at every step): X_traj 2nu x B x (T+1), Gx 2nu x 2nu x B x T, Gu 2nu x nu x B x T"
+function rollout_minimal_gradients(mech::Mechanism, X0::Matrix{Float64}, U::Array{Float64,3}; opts = SolverOptions{Float64}())
+    h = handle(mech); B = size(X0, 2); T = size(U, 3); nm = 2 * h.nu
+    Xt = zeros(nm, B, T + 1); Gx = zeros(nm, nm, B, T); Gu = zeros(nm, h.nu, B, T); status = zeros(Int32, B, T); iters = zeros(Int32, B, T)
+    rc = ccall((:dojo_rollout_minimal_gradients, LIB), Cint,
+               (Ptr{Cvoid}, Ref{COptions}, Cint, Cint, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}, Ptr{Int32}),
+               h.ptr, COptions(opts), B, T, X0, U, Xt, Gx, Gu, status, iters)
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return Xt, Gx, Gu, status
+end
+
 # ---- multi-GPU: one Julia process per GPU (e.g. MPI.jl ranks or Distributed workers); the exchange of the next states is fused into
 # the step kernel (peer writes over NVLink, include/dojo_b200.h "Multi-GPU"): no NCCL.jl needed.  `allgather_bytes` is any host-side
 # all-gather of a 128-byte blob per rank (MPI.Allgather, a shared file, ...), used ONCE at set-up.

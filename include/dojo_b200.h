@@ -19,6 +19,8 @@
  *                                                                  src/gradients/state.jl:69-126
  *   dojo_rollout                 <- simulate!(mechanism, steps, storage, control!)
  *                                                                  src/simulation/simulate.jl:16-36
+ *   dojo_rollout_grad            <- simulate! + get_maximal_gradients! at every step
+ *   dojo_rollout_minimal_gradients <- simulate! + get_minimal_gradients! at every step
  *   DojoSolverOptions            <- SolverOptions{T}               src/solver/options.jl:16-26
  *   dojo_minimal_to_maximal      <- minimal_to_maximal(mechanism, x) src/mechanism/state.jl:9-22
  *                                   (set_minimal_coordinates_velocities!, src/joints/minimal.jl:148-203)
@@ -320,6 +322,27 @@ int dojo_minimal_to_maximal_jacobian_async(DojoHandle* h, int B, const double* d
  * X [2 nu x B], U [nu x B] (nullable), X_next [2 nu x B]; status / iters nullable; host or device pointers. */
 int dojo_minimal_gradients(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* X, const double* U,
                            double* X_next, double* Gx, double* Gu, int32_t* status, int32_t* iters);
+
+/* Trajectory Jacobians: simulate! (src/simulation/simulate.jl:16-36) + get_maximal_gradients! (src/gradients/state.jl:69-126)
+ * at every step, i.e. (dz_{t+1}/dz_t, dz_{t+1}/du_t) for t = 0 .. T-1, the Jacobians of dojo_step_grad (consistent IFT, SURVEY Q2)
+ * at the states of the fused rollout of dojo_rollout.  Pair (e, t) is at index t*B + e.
+ *   Z_traj [13Nb x B x (T+1)]: slab 0 = Z0 on return, slab t+1 = state after step t (slab T = final state);
+ *   Fz [12Nb x 12Nb x B x T], Fu [12Nb x nu x B x T], column-major per pair as dojo_step_grad;
+ *   U [nu x B x T] nullable (zero input); status / iters [B x T] nullable: status and Newton iterations of every step.
+ * B in 1..max_batch, T >= 1 (DOJO_EINVAL otherwise); DOJO_ENOMEM when the gradient workspace does not fit (as dojo_step_grad).
+ * dojo_rollout_grad: host or device pointers (all of the same kind); host Jacobians are computed and copied in chunks of pairs.
+ * dojo_rollout_grad_async: device pointers, no synchronisation; the gradients of early steps are computed while later steps are
+ * still being solved.  Z_traj may hold Z0 in slab 0 already (dZ0 == dZ_traj). */
+int dojo_rollout_grad(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const double* U,
+                      double* Z_traj, double* Fz, double* Fu, int32_t* status, int32_t* iters);
+int dojo_rollout_grad_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU,
+                            double* dZ_traj, double* dFz, double* dFu, int32_t* dstatus, int32_t* diters, void* cuda_stream);
+/* The same in minimal coordinates: simulate! + get_minimal_gradients! (src/gradients/state.jl:182-217) at every step.  The rollout
+ * runs in maximal coordinates from minimal_to_maximal(X0); X_traj [2nu x B x (T+1)] is maximal_to_minimal of its T + 1 slabs,
+ * Gx [2nu x 2nu x B x T] = M(z_{t+1}) Fz N(z_t), Gu [2nu x nu x B x T] = M(z_{t+1}) Fu per pair (as dojo_minimal_gradients, whose
+ * maximal states never leave the device).  Host or device pointers (all of the same kind). */
+int dojo_rollout_minimal_gradients(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* X0, const double* U,
+                                   double* X_traj, double* Gx, double* Gu, int32_t* status, int32_t* iters);
 
 /* Batched environment layer (DojoEnvironments/src/environments.jl:77-109 and environments/{ant_ars,quadruped_sampling,
  * pendulum}.jl): state_map / input_map / step! / get_state plus the reward and failure test of the learning examples
