@@ -248,6 +248,21 @@ extern "C" void dojo_default_options(DojoSolverOptions* o) {
   o->undercut = INFINITY; o->no_progress_max = 3; o->no_progress_undercut = 10.0; o->verbose = 0;
 }
 
+// Gives a kernel function the most dynamic shared memory the device allows (the opt-in maximum minus the kernel's static shared
+// memory) and the max-shared carve-out.  The attributes belong to the kernel FUNCTION (per device), not to a handle: several handles
+// (ant, pendulum, ...) share the kernel symbols, so they are set to the device's maximum once and for all -- a handle created later
+// with a smaller arena must not lower them under the launches of an earlier, larger one
+// (tests/test_gpu_parity.py::test_two_handles_share_kernels).
+static cudaError_t max_shared_memory(const void* fn, int device) {
+  int optin = 0;
+  cudaFuncAttributes fa;
+  cudaError_t e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, fn);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  return e;
+}
+
 // [hostemu:padmask:begin]
 static void pad_mask(const DojoJointElementDesc& e, double* C, double* A) {
   // joints/joint.jl:56-64 (constraint_mask / nullspace_mask), zero-padded to 3 rows
@@ -705,24 +720,14 @@ extern "C" int dojo_create(const DojoMechanismDesc* d, int device, int max_batch
   h->small_step = small_step_ok(h, h->plan_smem_mask);
   h->k_fwd = step_kernel_fn(h->any_contact, false, h->plan_smem_mask == 0xff, h->small_step);
   h->k_grad = step_kernel_fn(h->any_contact, true, false);  // re-selected below once the gradient configuration is known
-  // The attribute belongs to the kernel FUNCTION (per device), not to this handle: several handles (ant, pendulum, ...) share the
-  // four kernel symbols, so it is set to the device's opt-in maximum once and for all -- a handle created later with a smaller
-  // arena must not lower it under the launches of an earlier, larger one (tests/test_gpu_parity.py::test_two_handles_share_kernels).
-  auto max_dynamic_smem = [&](const void* fn) {  // opt-in maximum minus the kernel's static shared memory
-    cudaFuncAttributes fa;
-    if (cudaFuncGetAttributes(&fa, fn) != cudaSuccess) { ok = false; return; }
-    ok = ok && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(prop.sharedMemPerBlockOptin - fa.sharedSizeBytes)) == cudaSuccess;
-  };
-  max_dynamic_smem(h->k_fwd);
-  ok = ok && cudaFuncSetAttribute(h->k_fwd, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) == cudaSuccess;
+  ok = ok && max_shared_memory(h->k_fwd, device) == cudaSuccess;
   const bool grad_fits = h->grad_bytes <= (size_t)prop.sharedMemPerBlockOptin;
   if (grad_fits) {
     h->slots_grad = pick_slots(h->grad_bytes);
     plan_prefix(h->slots_grad, h->grad_bytes, &h->plan_smem_off_grad, &h->plan_smem_bytes_grad, &h->plan_smem_mask_grad);
     h->smem_grad = h->slots_grad * h->grad_bytes + h->plan_smem_bytes_grad;
     h->k_grad = step_kernel_fn(h->any_contact, true, h->plan_smem_mask_grad == 0xff);
-    max_dynamic_smem(h->k_grad);
-    ok = ok && cudaFuncSetAttribute(h->k_grad, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) == cudaSuccess;
+    ok = ok && max_shared_memory(h->k_grad, device) == cudaSuccess;
   } else h->grad_bytes = 0;
   if (!ok) { g_create_error = std::string("dojo_create: device allocation failed: ") + cudaGetErrorString(cudaGetLastError()); dojo_destroy(h); return DOJO_ECUDA; }
   // the device code reaches the tables through Ctx (shared-memory copy or this blob); the Plan pointers are kept for debugging
@@ -798,11 +803,25 @@ static Options make_options(const DojoSolverOptions* o) {
 }
 // [hostemu:options:end]
 
+// The kernel arguments every launch starts from: all zero, except the plan, the solver options, the batch, one time step, the handle's
+// work-queue counter and profile counters, and where the plan tables lie in the forward or (grad) the gradient launch configuration
+static StepArgs step_args(const DojoHandle* h, const DojoSolverOptions* opts, int B, bool grad) {
+  StepArgs a = {};
+  a.plan = h->plan; a.opts = make_options(opts); a.B = B; a.T = 1;
+  a.counter = h->d_counter; a.prof = h->d_prof;
+  a.slot_stride = (int)((grad ? h->grad_bytes : h->arena_bytes) / sizeof(double));
+  a.plan_blob = h->d_blob; a.plan_bytes = h->blob_bytes;
+  a.plan_smem_off = grad ? h->plan_smem_off_grad : h->plan_smem_off;
+  a.plan_smem_bytes = grad ? h->plan_smem_bytes_grad : h->plan_smem_bytes;
+  a.plan_smem_mask = grad ? h->plan_smem_mask_grad : h->plan_smem_mask;
+  for (int k = 0; k < 8; ++k) a.plan_off[k] = h->blob_off[k];
+  return a;
+}
+
 static int launch_forward(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ, const double* dU, const double* dFext, double* dZn, double* dsol,
                           double* dsol_raw, int32_t* dstatus, int32_t* diters, uint32_t flags, cudaStream_t s, int* done_count = nullptr, int* done_list = nullptr,
                           DojoGather* g = nullptr, double* dtrace = nullptr) {
-  StepArgs a;
-  a.n_peers = 0; a.gather_off = 0;
+  StepArgs a = step_args(h, opts, B, false);
   a.trace = dtrace;  // non-null: the traced kernel (dojo_step_trace_async)
   if (g) {
     if (!g->connected || g->h != h || B != g->B) { h->err = "dojo_step_gather_async: gather not connected / made for another handle / B differs from B_local"; return DOJO_EINVAL; }
@@ -811,10 +830,8 @@ static int launch_forward(DojoHandle* h, const DojoSolverOptions* opts, int B, c
     g->last = g->parity; g->parity ^= 1;
     for (int r = 0; r < g->world; ++r) { a.peer_buf[r] = g->peer_buf[r]; a.peer_flag[r] = g->peer_flag[r]; }
   }
-  a.plan = h->plan; a.opts = make_options(opts); a.B = B;
   a.Z = dZ; a.U = dU; a.Fext = dFext; a.Zn = dZn; a.sol = dsol; a.sol_raw = dsol_raw; a.status = dstatus; a.iters = diters; a.flags = flags;
-  a.Fz = nullptr; a.Fu = nullptr; a.Fc = nullptr; a.T = 1; a.traj = nullptr; a.done_count = done_count; a.done_list = done_list;
-  a.counter = h->d_counter;
+  a.done_count = done_count; a.done_list = done_list;
   // LPT order from the previous call's iteration counts (only meaningful when the same batch is stepped again, which is what
   // simulation loops do; a stale order is harmless -- it is just an order)
   enter_call(h, s);
@@ -831,11 +848,7 @@ static int launch_forward(DojoHandle* h, const DojoSolverOptions* opts, int B, c
     CUDA_TRY(h, cudaGetLastError());
     h->launches += 1;
   }
-  a.prof = h->d_prof;
   CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
-  a.slot_stride = (int)(h->arena_bytes / sizeof(double));
-  a.plan_blob = h->d_blob; a.plan_bytes = h->blob_bytes; a.plan_smem_off = h->plan_smem_off; a.plan_smem_bytes = h->plan_smem_bytes; a.plan_smem_mask = h->plan_smem_mask;
-  for (int k = 0; k < 8; ++k) a.plan_off[k] = h->blob_off[k];
   int grid = std::min((B + h->slots - 1) / h->slots, h->sm_count * h->envs_per_sm);
   const void* k = dtrace ? h->k_fwd_trace : h->k_fwd;
   { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(k, dim3(grid), dim3(32 * h->nw * h->slots), kargs, h->smem_fwd, s)); }
@@ -891,12 +904,7 @@ static int ensure_staging(DojoHandle* h) {
 static int ensure_trace_kernel(DojoHandle* h) {
   if (h->k_fwd_trace) return DOJO_OK;
   const void* k = step_trace_kernel_fn(h->any_contact, h->plan_smem_mask == 0xff);
-  int optin = 0;
-  cudaFuncAttributes fa;
-  CUDA_TRY(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-  CUDA_TRY(h, cudaFuncGetAttributes(&fa, k));
-  CUDA_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
-  CUDA_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  CUDA_TRY(h, max_shared_memory(k, h->device));
   h->k_fwd_trace = k;
   return DOJO_OK;
 }
@@ -992,17 +1000,11 @@ extern "C" int dojo_step_trace(DojoHandle* h, const DojoSolverOptions* opts, int
 static int launch_rollout(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZf, double* dtraj,
                           int32_t* dstatus, cudaStream_t s, int32_t* diters = nullptr, double* dsol_raw = nullptr, int* done_count = nullptr,
                           int* done_list = nullptr) {
-  StepArgs a;
-  a.plan = h->plan; a.opts = make_options(opts); a.B = B;
-  a.Z = dZ0; a.U = dU; a.Fext = nullptr; a.Zn = dZf; a.sol = nullptr; a.sol_raw = dsol_raw; a.status = dstatus; a.iters = diters; a.flags = 0;
-  a.Fz = nullptr; a.Fu = nullptr; a.Fc = nullptr; a.T = T; a.traj = dtraj; a.done_count = done_count; a.done_list = done_list;
-  a.counter = h->d_counter; a.prof = h->d_prof; a.order = nullptr; a.prev_iters = nullptr;
-  a.n_peers = 0; a.gather_off = 0; a.trace = nullptr;
+  StepArgs a = step_args(h, opts, B, false);
+  a.Z = dZ0; a.U = dU; a.Zn = dZf; a.sol_raw = dsol_raw; a.status = dstatus; a.iters = diters;
+  a.T = T; a.traj = dtraj; a.done_count = done_count; a.done_list = done_list;
   enter_call(h, s);
   CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
-  a.slot_stride = (int)(h->arena_bytes / sizeof(double));
-  a.plan_blob = h->d_blob; a.plan_bytes = h->blob_bytes; a.plan_smem_off = h->plan_smem_off; a.plan_smem_bytes = h->plan_smem_bytes; a.plan_smem_mask = h->plan_smem_mask;
-  for (int k = 0; k < 8; ++k) a.plan_off[k] = h->blob_off[k];
   const bool rec = dsol_raw != nullptr;
   int grid = std::min((B + h->slots - 1) / h->slots, h->sm_count * (rec ? h->envs_per_sm_rec : h->envs_per_sm));
   { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(rec ? h->k_fwd_rec : h->k_fwd, dim3(grid), dim3(32 * h->nw * h->slots), kargs, h->smem_fwd, s)); }
@@ -1120,17 +1122,11 @@ static int step_grad_impl(DojoHandle* h, const DojoSolverOptions* opts, int B, c
 static int launch_grad(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* dZ, const double* dU, const double* dFext, double* dsol_raw,
                        int32_t* dstatus, double* dFz, double* dFu, double* dFc, uint32_t flags, int* done_list, int* counter, cudaStream_t s) {
   const bool overlap = done_list != nullptr;
-  StepArgs a;
-  a.plan = h->plan; a.opts = make_options(opts); a.B = B;
-  a.Z = dZ; a.U = dU; a.Fext = dFext; a.Zn = nullptr; a.sol = nullptr; a.sol_raw = dsol_raw; a.status = dstatus; a.iters = nullptr; a.flags = flags;
-  a.Fz = dFz; a.Fu = dFu; a.Fc = dFc; a.T = 1; a.traj = nullptr; a.done_count = nullptr; a.done_list = done_list;
-  a.n_peers = 0; a.gather_off = 0; a.trace = nullptr;
-  a.counter = overlap ? counter : h->d_counter; a.order = nullptr; a.prev_iters = nullptr;
-  a.prof = h->d_prof;
-  if (!overlap) CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
-  a.slot_stride = (int)(h->grad_bytes / sizeof(double));
-  a.plan_blob = h->d_blob; a.plan_bytes = h->blob_bytes; a.plan_smem_off = h->plan_smem_off_grad; a.plan_smem_bytes = h->plan_smem_bytes_grad; a.plan_smem_mask = h->plan_smem_mask_grad;
-  for (int k = 0; k < 8; ++k) a.plan_off[k] = h->blob_off[k];
+  StepArgs a = step_args(h, opts, B, true);
+  a.Z = dZ; a.U = dU; a.Fext = dFext; a.sol_raw = dsol_raw; a.status = dstatus; a.flags = flags;
+  a.Fz = dFz; a.Fu = dFu; a.Fc = dFc; a.done_list = done_list;
+  if (overlap) a.counter = counter;
+  else CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
   int grid = std::min((B + h->slots_grad - 1) / h->slots_grad, h->sm_count * h->envs_per_sm_grad);
   if (overlap) {
     cudaLaunchConfig_t cfg = {};
@@ -1533,12 +1529,8 @@ extern "C" int dojo_minimal_gradients(DojoHandle* h, const DojoSolverOptions* op
 static int ensure_rec_kernel(DojoHandle* h) {
   if (h->k_fwd_rec) return DOJO_OK;
   const void* k = step_rec_kernel_fn(h->any_contact, h->plan_smem_mask == 0xff);
-  int optin = 0, occ = 1;
-  cudaFuncAttributes fa;
-  CUDA_TRY(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-  CUDA_TRY(h, cudaFuncGetAttributes(&fa, k));
-  CUDA_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
-  CUDA_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  int occ = 1;
+  CUDA_TRY(h, max_shared_memory(k, h->device));
   CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, 32 * h->nw * h->slots, h->smem_fwd));
   h->envs_per_sm_rec = std::max(1, occ);
   h->k_fwd_rec = k;

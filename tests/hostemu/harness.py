@@ -14,7 +14,8 @@ def _p(a):
 
 
 class HostEmu:
-    """The product's dojo_step_kernel<false/true> run on CPU fibers for one mechanism."""
+    """The product's dojo_step_kernel<false/true> run on CPU fibers for one mechanism.  The ctypes signatures of every entry point of
+    driver.inc are declared here, also those that only the subclasses in trace.py, small.py and rollout_grad.py call."""
 
     def __init__(self, mech):
         L = C.CDLL(gen.build())
@@ -30,6 +31,10 @@ class HostEmu:
         L.hostemu_step.argtypes = [_vp, op, _ip, _ip, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint32, _ip, _ip, _ip, _vp]
         L.hostemu_step_grad.argtypes = [_vp, op, _ip, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ip, _ip, _ip, _ip, _vp]
         L.hostemu_kinjac.argtypes = [_vp, _ip, _ip, _ip, _vp, _vp, _vp, _vp, _vp, _vp]
+        L.hostemu_step_trace.argtypes = [_vp, op, _ip, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint32, _ip, _ip, _ip]
+        L.hostemu_step_small.argtypes = [_vp, op, _ip, _ip, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint32, _ip, _ip, _vp]
+        L.hostemu_small_step_ok.argtypes = [_vp, _ip]
+        L.hostemu_rollout_grad.argtypes = [_vp, op, _ip, _ip, _vp, _vp, _vp, _vp, _vp, _vp, _ip, _ip, _ip, _ip]
         self.L, self.mech = L, mech
         desc, self._keep = capi.flatten(mech)
         h = L.hostemu_create(C.byref(desc))

@@ -1,46 +1,28 @@
 """The traced step on the CPU -- TEST INFRASTRUCTURE for tests/test_solver_trace.py and tests/test_zzzzz_gpu_solver_trace.py.
 
-Two builds of existing test infrastructure, each generated from its unmodified source the way gen.py builds the kernel emulation:
-
-  * TracedEmu: the kernel emulation TU of gen.py plus one more entry point, hostemu_step_trace, which runs the product's traced kernel
-    dojo_step_kernel<false, false, true> on CPU fibers (the other entry points of driver.inc stay as they are).
+  * TracedEmu: the kernel emulation (gen.py) through its entry point hostemu_step_trace (driver.inc), which runs the product's traced
+    kernel dojo_step_kernel<false, false, true> on CPU fibers.
   * TracedOracle: the CPU oracle (oracle/dojo_oracle.cpp) with its loop-head record extended by a fifth column, the trials the previous
     iteration's line_search evaluated up to and including the accepted one, so that its rows can be compared with the device's
     [rvio, bvio, alpha, mu, trials] (include/dojo_b200.h, dojo_step_trace).  Five textual substitutions, each asserted to apply exactly
-    once; they add integer bookkeeping only, and the tests check that its steps stay bit-identical to the oracle's.
-
-Both libraries are built into tests/hostemu/_build (or a temporary directory when the tree is read-only)."""
+    once; they add integer bookkeeping only, and the tests check that its steps stay bit-identical to the oracle's.  Built from the
+    unmodified source into the emulation's build directory (gen.build_dir)."""
 import ctypes as C
 import os
 import subprocess
-import tempfile
 
 import numpy as np
 
 from dojo_jl_b200 import capi
 from oracle import oracle as _oracle
 from . import gen
-from .harness import HostEmu, _ip, _p, _vp
+from .harness import HostEmu, _p
 
 ROOT = gen.ROOT
 ORACLE_DIR = os.path.join(ROOT, "oracle")
 
 
-def _build_dir():
-    d = gen.BUILD
-    try:
-        os.makedirs(d, exist_ok=True)
-        if os.access(d, os.W_OK):
-            return d
-    except OSError:
-        pass
-    d = os.path.join(tempfile.gettempdir(), "dojo_hostemu_trace_%d" % os.getuid())
-    os.makedirs(d, exist_ok=True)
-    return d
-
-
-def _stale(lib, deps):
-    return not os.path.exists(lib) or any(os.path.getmtime(d) > os.path.getmtime(lib) for d in deps)
+_build_dir, _stale = gen.build_dir, gen.stale
 
 
 def _compile(src_text, name, cmd):
@@ -63,57 +45,8 @@ def _substitute(text, subs, what):
 
 
 # ---------------------------------------------------------------------------------------------------------------- kernel emulation
-_EMU_ENTRY = r"""
-// dojo_step_trace on the emulation: the traced kernel, trace [5 x max_iter x B]
-extern "C" int hostemu_step_trace(void* p, const DojoSolverOptions* opts, int B, const double* Z, const double* U, const double* Fext, double* Zn,
-                                  double* sol, int32_t* status, int32_t* iters, double* trace, uint32_t flags, int slots, int smem_plan, int grid) {
-  DojoHandle* h = static_cast<EmuHandle*>(p)->h;
-  int counter = 0;
-  StepArgs a = emu_args(h, opts, B, false, slots, smem_plan != 0, &counter);
-  a.Z = Z; a.U = U; a.Fext = Fext; a.Zn = Zn; a.sol = sol; a.status = status; a.iters = iters; a.flags = flags; a.trace = trace;
-  const size_t smem = slots * h->arena_bytes + (smem_plan ? h->blob_bytes : 0);
-  for (int b = 0; b < grid; ++b) emu::run_cta(b, grid, 32 * h->nw * slots, smem, [&a] { dojo_step_kernel<false, false, true>(a); });
-  return 0;
-}
-"""
-
-
-def build_emulation() -> str:
-    name = "libdojo_hostemu_trace_fma.so" if gen.FMA else "libdojo_hostemu_trace.so"
-    lib = os.path.join(_build_dir(), name)
-    if not _stale(lib, gen.DEPS + [os.path.abspath(__file__)]):
-        return lib
-    here = gen.HERE
-    text = open(gen.generate()).read()
-    text = _substitute(text, [('#include "../cuda_shim.h"', f'#include "{os.path.join(here, "cuda_shim.h")}"'),
-                              ('#include "../driver.inc"', f'#include "{os.path.join(here, "driver.inc")}"')], "the emulation TU")
-    fp = ["-ffp-contract=fast", "-march=x86-64-v3"] if gen.FMA else ["-ffp-contract=off"]
-    cmd = ["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared"] + fp + ["-Wno-unknown-pragmas", "-Wno-unused-function", "-Wno-unused-variable",
-                                                                         "-Wno-unused-but-set-variable"]
-    return _compile(text + _EMU_ENTRY, name, cmd)
-
-
 class TracedEmu(HostEmu):
-    """HostEmu's untraced step (step) and the traced one (step_trace) on the library that carries both kernels."""
-
-    def __init__(self, mech):
-        L = C.CDLL(build_emulation())
-        L.hostemu_step_trace.argtypes = [_vp, C.POINTER(capi.DojoSolverOptions), _ip, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint32, _ip, _ip, _ip]
-        L.hostemu_step_trace.restype = C.c_int
-        L.hostemu_create.restype = _vp
-        L.hostemu_create.argtypes = [C.POINTER(capi.DojoMechanismDesc)]
-        L.hostemu_destroy.argtypes = [_vp]
-        L.hostemu_last_error.restype = C.c_char_p
-        L.hostemu_num_residual.argtypes = [_vp]
-        op = C.POINTER(capi.DojoSolverOptions)
-        L.hostemu_step.argtypes = [_vp, op, _ip, _ip, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint32, _ip, _ip, _ip, _vp]
-        self.L, self.mech = L, mech
-        desc, self._keep = capi.flatten(mech)
-        h = L.hostemu_create(C.byref(desc))
-        if not h:
-            raise RuntimeError("hostemu_create failed: " + L.hostemu_last_error().decode())
-        self.h = C.c_void_p(h)
-        assert L.hostemu_num_residual(self.h) == mech.nres
+    """HostEmu's untraced step (step) and the traced one (step_trace)."""
 
     def step_trace(self, Z, U=None, opts=None, fext=None, flags=0, slots=1, smem_plan=True, grid=1):
         """dojo_step_trace.  Returns (Z_next, status, iters, sol, trace [B, max_iter, 5])."""
