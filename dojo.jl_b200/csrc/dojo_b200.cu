@@ -638,6 +638,48 @@ extern "C" int dojo_create(const DojoMechanismDesc* d, int device, int max_batch
   }
   P.nphase = nphase;
   h->nsteps = (int)steps.size();
+  {  // ---- the LDU program (dojo_plan.h LduOp), appended to the schedule table
+    std::vector<int> cnt((size_t)nphase * nw), wfirst(nw);
+    std::vector<LduOp> ops;
+    bool fits = true;  // every offset below kLduNone, every size below 256
+    auto u16 = [&](int v) { fits = fits && v >= 0 && v < kLduNone; return v & 0xffff; };
+    auto u8 = [&](int v) { fits = fits && v >= 0 && v < 256; return v & 0xff; };
+    for (int w = 0; w < nw; ++w) {
+      wfirst[w] = (int)ops.size();
+      for (int ph = 0; ph < nphase; ++ph) {
+        const int s0 = sched[2 * (ph * nw + w)], sn = sched[2 * (ph * nw + w) + 1];
+        cnt[ph * nw + w] = sn;
+        for (int s = s0; s < s0 + sn; ++s) {
+          const ElimStep& st = steps[s];
+          int f[kLduFold] = {0, 0, 0};
+          for (int k = 0; k < std::min(st.fold_cnt, kLduFold); ++k) f[k] = ilist[st.fold_off + k];
+          LduOp op;
+          std::memset(&op, 0, sizeof(op));
+          op.w[0] = u16(st.d_off) | u16(st.vec_off) << 16;
+          op.w[1] = u8(st.n) | u8(st.nnb) << 8 | u16(st.fold_cnt) << 16;
+          op.w[2] = u16(st.fold_off) | u16(f[0]) << 16;
+          op.w[3] = u16(f[1]) | u16(f[2]) << 16;
+          for (int i = 0; i < st.nnb; ++i) {
+            const ElimNb& nb = st.nb[i];
+            int* q = op.w + 4 * (1 + i);
+            q[0] = u16(nb.L_off) | (nb.fwd_abs >= 0 ? u16(nb.fwd_abs) : kLduNone) << 16;
+            q[1] = u16(nb.vec_off) | u16(nb.U_off) << 16;
+            q[2] = u8(nb.n) | u8(nb.U_row) << 8 | u8(nb.U_k) << 16 | u8(nb.ld) << 24;
+            q[3] = u16(st.tgt[i][0]) | (st.nnb > 1 ? u16(st.tgt[i][1]) : 0) << 16;
+          }
+          ops.push_back(op);
+        }
+      }
+    }
+    if (!fits) { delete h; return fail("the block LDU program does not fit its 16-bit offsets"); }
+    P.prog_cnt = (int)sched.size();
+    sched.insert(sched.end(), cnt.begin(), cnt.end());
+    sched.insert(sched.end(), wfirst.begin(), wfirst.end());
+    sched.resize((sched.size() + 3) & ~size_t(3), 0);  // the ops start on a 16-byte boundary of the (16-byte aligned) table
+    P.prog_ops = (int)sched.size();
+    const int* words = reinterpret_cast<const int*>(ops.data());
+    sched.insert(sched.end(), words, words + ops.size() * (sizeof(LduOp) / sizeof(int)));
+  }
   // [hostemu:tables:end]
 
   // ---- device resources
@@ -660,10 +702,11 @@ extern "C" int dojo_create(const DojoMechanismDesc* d, int device, int max_batch
     const void* src[8] = {bodies.data(), joints.data(), contacts.data(), steps.data(), sched.data(), ilist.data(), roles.data(), ucol.data()};
     const size_t len[8] = {sizeof(BodyDev) * Nb, sizeof(JointDev) * Ne, sizeof(ContactDev) * Ni, sizeof(ElimStep) * steps.size(), sizeof(int) * sched.size(),
                            sizeof(int) * ilist.size(), sizeof(WarpRole) * roles.size(), sizeof(int) * ucol.size()};
-    // physical order: the tables walked by the serial phases of the solver (elimination steps, schedule, lists, roles) first, the
-    // per-node descriptors (read by one lane per node) last, so that a PREFIX of the blob can ride in shared memory when the whole
-    // does not fit behind the arenas (quadruped: 4 x 56.7 KB leave 5.6 KB)
-    const int order[8] = {3, 4, 5, 6, 7, 0, 2, 1};
+    // physical order: the tables walked by the serial phases of the solver (schedule with the LDU program, elimination steps, lists,
+    // roles) first, the per-node descriptors (read by one lane per node) last, so that a PREFIX of the blob can ride in shared memory
+    // when the whole does not fit behind the arenas (atlas: 2 x 102.5 KiB leave 21 KiB, quadruped's gradient pass 2 x 108.4 KiB leave
+    // 9.2 KiB)
+    const int order[8] = {4, 3, 5, 6, 7, 0, 2, 1};
     for (int q = 0; q < 8; ++q) {
       const int k = order[q];
       h->blob_off[k] = (int)blob.size();

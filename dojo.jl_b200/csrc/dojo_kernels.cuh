@@ -79,6 +79,7 @@ struct Ctx {
 #ifdef DJ_PROFILE
   long long t_eval_jac, t_eval_ls, t_fact, t_solve, t_misc, t_align, t_cone, t_center, t_rolewait, t_last;
   long long f_fold, f_inv, f_rm, f_schur, f_bar, f_last;
+  long long s_cond, s_fwd, s_bwd, s_rec, s_bar;  // solve(): condense + gather, forward sweep, backward sweep, recover, slot barriers
 #endif
 };
 #ifdef DJ_PROFILE
@@ -1302,6 +1303,15 @@ DJ_DEV void evaluate_ls(Ctx& c, double* W, double fk, bool pair, double& rvA, do
 // ------------------------------------------------------------------------------------------------------------
 // Block LDU (GraphBasedSystems.ldu_factorization! / ldu_backsubstitution!), phase-parallel over the warps
 // ------------------------------------------------------------------------------------------------------------
+// The LDU program of the plan (dojo_plan.h LduOp): cnt[ph * nw + w] and, after them, wfirst[w]; op k is three 16-byte words
+DJ_DEV const int* ldu_cnt(const Ctx& c) { return c.sched + c.P->prog_cnt; }
+DJ_DEV const int4* ldu_op(const Ctx& c, int k) { return reinterpret_cast<const int4*>(c.sched + c.P->prog_ops) + 3 * k; }
+// arena offset of the j-th scratch record folded into the step of op word 0 `h` (the first kLduFold are inline)
+DJ_DEV int ldu_fold(const Ctx& c, int4 h, int j) {
+  return j == 0 ? hi16(h.z) : j == 1 ? lo16(h.w) : j == 2 ? hi16(h.w) : c.ilist[lo16(h.z) + j];
+}
+static_assert(kLduFold == 3, "ldu_fold names three inline fold sources");
+
 template <bool SMALL = false>
 DJ_DEV bool factorize(Ctx& c) {
   const Plan& P = *c.P;
@@ -1310,33 +1320,44 @@ DJ_DEV bool factorize(Ctx& c) {
   // the two halves of a warp eliminate two steps of the phase at the same time (blocks are at most 6 x 6: 12 lanes busy)
   const int half = c.lane >> 4, l = c.lane & 15;
   const unsigned mask = 0xffffu << (16 * half);
+  const int nw = slot_warps<SMALL>(c);
+  const int* cnt = ldu_cnt(c);
+  int k = cnt[P.nphase * nw + c.warp];  // this warp's first op of the phase
 #ifdef DJ_PROFILE
   c.f_last = clock64();
 #endif
   for (int ph = 0; ph < P.nphase; ++ph) {
-    const int s0 = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp)], sn = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp) + 1];
-    for (int s = s0 + half; s < s0 + sn; s += 2) {
-      const ElimStep& st = c.steps[s];
-      double* Dc = A + st.d_off;
-      if (st.fold_cnt > 0) {  // fold the children's scratch updates into D_c
-        for (int t = l; t < st.n * st.n; t += 16) {
+    const int sn = cnt[ph * nw + c.warp];
+    for (int s = half; s < sn; s += 2) {
+      const int4* q = ldu_op(c, k + s);
+      const int4 h = q[0];
+      const int n = byte_of(h.y, 0), nnb = byte_of(h.y, 1), fold_cnt = hi16(h.y);
+      double* Dc = A + lo16(h.x);
+      if (fold_cnt > 0) {  // fold the children's scratch updates into D_c
+        for (int t = l; t < n * n; t += 16) {
           double acc = Dc[t];
-          for (int k = 0; k < st.fold_cnt; ++k) acc += A[c.ilist[st.fold_off + k] + t];
+          for (int j = 0; j < fold_cnt; ++j) acc += A[ldu_fold(c, h, j) + t];
           Dc[t] = acc;
         }
         __syncwarp(mask);
       }
       DJ_FTICK(c, f_fold)
-      ok = block_inverse(Dc, st.n, st.n, l, mask) && ok;                                                  // D_c <- D_c^-1
+      ok = block_inverse(Dc, n, n, l, mask) && ok;                                                        // D_c <- D_c^-1
       DJ_FTICK(c, f_inv)
-      for (int i = 0; i < st.nnb; ++i) right_multiply_inplace(A + st.nb[i].L_off, Dc, st.nb[i].n, st.n, l, mask);  // L~_ic = M_ic D_c^-1
+      for (int i = 0; i < nnb; ++i) {                                                                     // L~_ic = M_ic D_c^-1
+        const int4 a = q[1 + i];
+        right_multiply_inplace(A + lo16(a.x), Dc, byte_of(a.z, 0), n, l, mask);
+      }
       DJ_FTICK(c, f_rm)
-      for (int i = 0; i < st.nnb; ++i)
-        for (int j = 0; j < st.nnb; ++j)                                                                  // M_ij -= L~_ic M_cj
-          schur_update(A + st.tgt[i][j], st.nb[j].ld, A + st.nb[i].L_off + st.nb[j].U_row, st.n, A + st.nb[j].U_off, st.nb[i].n, st.nb[j].U_k,
-                       st.nb[j].n, l, mask);
+      for (int i = 0; i < nnb; ++i)
+        for (int j = 0; j < nnb; ++j) {                                                                   // M_ij -= L~_ic M_cj
+          const int4 ai = q[1 + i], aj = q[1 + j];
+          schur_update(A + (j ? hi16(ai.w) : lo16(ai.w)), byte_of(aj.z, 3), A + lo16(ai.x) + byte_of(aj.z, 1), n, A + hi16(aj.y), byte_of(ai.z, 0),
+                       byte_of(aj.z, 2), byte_of(aj.z, 0), l, mask);
+        }
       DJ_FTICK(c, f_schur)
     }
+    k += sn;
     slot_sync(c);
     DJ_FTICK(c, f_bar)
   }
@@ -1373,6 +1394,9 @@ DJ_DEV void solve(Ctx& c, int vec_off) {
   const int half = lane >> 4, l = lane & 15;  // one elimination step per half-warp, as in factorize()
   const int sub = l >> 3, li = l & 7;         // forward substitution: lanes [0,8) of the group serve nb[0], [8,16) nb[1]
   const WarpRole& role = c.roles[c.warp];
+#ifdef DJ_PROFILE
+  c.f_last = clock64();
+#endif
   // condense the right-hand side of the contact / joint-limit rows onto the body rows
   for (int p = 0; p < role.npass; ++p) {
     const int idx = role_item(role, p, lane);
@@ -1380,7 +1404,9 @@ DJ_DEV void solve(Ctx& c, int vec_off) {
     if (role.type[p] == ROLE_CONTACT) condense_contact(c, idx, x);
     else if (role.type[p] == ROLE_JOINT) condense_joint(c, idx, x);
   }
+  DJ_FTICK(c, s_cond)
   slot_sync(c);
+  DJ_FTICK(c, s_bar)
   for (int p = 0; p < role.npass; ++p) {
     const int idx = role_item(role, p, lane);
     if (idx < 0 || role.type[p] != ROLE_BODY) continue;
@@ -1392,65 +1418,83 @@ DJ_DEV void solve(Ctx& c, int vec_off) {
       add3(xb + 3, ld3(s + 3));
     }
   }
+  DJ_FTICK(c, s_cond)
   slot_sync(c);
+  DJ_FTICK(c, s_bar)
   // The two halves of a warp take two steps of a phase with one instruction stream.  Both halves run the same number of loop
   // iterations (a half without a step of its own looks at its partner's and stores nothing), so the warp stays converged and the
   // intra-step synchronisation is the plain full-warp one: a __syncwarp / shuffle whose member mask DIFFERS between the lanes of one
   // instruction (one 16-lane mask per half) is split into groups with MATCH.ANY by the compiler, whose sequences stall the warp.
+  // The ops of this warp are walked with a running index k (its first op of the phase): up through the phases, then back down.
+  const int nw = slot_warps<SMALL>(c);
+  const int* cnt = ldu_cnt(c);
+  int k = cnt[P.nphase * nw + c.warp];
   for (int ph = 0; ph < P.nphase; ++ph) {  // forward: z_i -= L~_ic z_c
-    const int s0 = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp)], sn = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp) + 1];
+    const int sn = cnt[ph * nw + c.warp];
     for (int it = 0; 2 * it < sn; ++it) {
       const bool act = 2 * it + half < sn;
-      const ElimStep& st = c.steps[s0 + 2 * it + (act ? half : 0)];
-      double* xc = x + st.vec_off;
-      if (act && st.fold_cnt > 0 && l < st.n) {  // fold (and clear) the children's forward updates of this body
+      const int4* q = ldu_op(c, k + 2 * it + (act ? half : 0));
+      const int4 h = q[0];
+      const int n = byte_of(h.y, 0), fold_cnt = hi16(h.y);
+      double* xc = x + hi16(h.x);
+      if (act && fold_cnt > 0 && l < n) {  // fold (and clear) the children's forward updates of this body
         double acc = xc[l];
-        for (int k = 0; k < st.fold_cnt; ++k) {
-          double* v = A + c.ilist[st.fold_off + k] + 36;
+        for (int j = 0; j < fold_cnt; ++j) {
+          double* v = A + ldu_fold(c, h, j) + 36;
           acc += v[l];
           v[l] = 0.0;
         }
         xc[l] = acc;
       }
       __syncwarp();
-      if (act && sub < st.nnb && li < st.nb[sub].n) {
-        const ElimNb& nb = st.nb[sub];
-        const double* L = A + nb.L_off + li * st.n;
-        const double acc = dot6(L, xc, st.n);
-        double* tgt = nb.fwd_abs >= 0 ? A + nb.fwd_abs : x + nb.vec_off;
-        tgt[li] -= acc;
+      if (act && sub < byte_of(h.y, 1)) {
+        const int4 a = q[1 + sub];  // neighbour `sub`
+        if (li < byte_of(a.z, 0)) {
+          const double* L = A + lo16(a.x) + li * n;
+          const double acc = dot6(L, xc, n);
+          double* tgt = hi16(a.x) != kLduNone ? A + hi16(a.x) : x + lo16(a.y);
+          tgt[li] -= acc;
+        }
       }
       __syncwarp();
     }
+    k += sn;
+    DJ_FTICK(c, s_fwd)
     slot_sync(c);
+    DJ_FTICK(c, s_bar)
   }
   for (int ph = P.nphase - 1; ph >= 0; --ph) {  // backward: x_c = D_c^-1 (z_c - sum_j M_cj x_j)
-    const int s0 = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp)], sn = c.sched[2 * (ph * slot_warps<SMALL>(c) + c.warp) + 1];
     // same pairing as the forward sweep, last pair first (the steps of one phase are independent)
+    const int sn = cnt[ph * nw + c.warp];
+    k -= sn;
     for (int it = (sn + 1) / 2 - 1; it >= 0; --it) {
       const bool act = 2 * it + half < sn;
-      const ElimStep& st = c.steps[s0 + 2 * it + (act ? half : 0)];
-      const double* Dc = A + st.d_off;
-      double* xc = x + st.vec_off;
-      if (act && st.nnb > 0 && l < st.n) {
+      const int4* q = ldu_op(c, k + 2 * it + (act ? half : 0));
+      const int4 h = q[0];
+      const int n = byte_of(h.y, 0), nnb = byte_of(h.y, 1);
+      const double* Dc = A + lo16(h.x);
+      double* xc = x + hi16(h.x);
+      if (act && nnb > 0 && l < n) {
         double acc = 0.0;
-        for (int j = 0; j < st.nnb; ++j) {
-          const ElimNb& nb = st.nb[j];
-          int r = l - nb.U_row;
-          if (r >= 0 && r < nb.U_k) {
-            acc += dot6(A + nb.U_off + r * nb.n, x + nb.vec_off, nb.n);
+        for (int j = 0; j < nnb; ++j) {
+          const int4 a = q[1 + j];
+          const int nn = byte_of(a.z, 0), r = l - byte_of(a.z, 1);
+          if (r >= 0 && r < byte_of(a.z, 2)) {
+            acc += dot6(A + hi16(a.y) + r * nn, x + lo16(a.y), nn);
           }
         }
         xc[l] -= acc;
       }
       __syncwarp();
       double acc = 0.0;
-      if (act && l < st.n) acc = dot6(Dc + l * st.n, xc, st.n);
+      if (act && l < n) acc = dot6(Dc + l * n, xc, n);
       __syncwarp();
-      if (act && l < st.n) xc[l] = acc;
+      if (act && l < n) xc[l] = acc;
       __syncwarp();
     }
+    DJ_FTICK(c, s_bwd)
     slot_sync(c);
+    DJ_FTICK(c, s_bar)
   }
   // recover the condensed-out steps (ds, dgamma) of the contacts and joint limits
   for (int p = 0; p < role.npass; ++p) {
@@ -1459,7 +1503,9 @@ DJ_DEV void solve(Ctx& c, int vec_off) {
     if (role.type[p] == ROLE_CONTACT) recover_contact(c, idx, x);
     else if (role.type[p] == ROLE_JOINT) recover_joint(c, idx, x);
   }
+  DJ_FTICK(c, s_rec)
   slot_sync(c);
+  DJ_FTICK(c, s_bar)
 }
 
 // ------------------------------------------------------------------------------------------------------------

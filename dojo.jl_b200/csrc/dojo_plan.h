@@ -131,6 +131,28 @@ struct ElimStep {
   int fold_off, fold_cnt;  // scratch records (Plan::ilist) folded into (D_c, z_c) before c is eliminated
 };
 
+// The block LDU of the Newton loop (factorize / solve) reads its steps from a flat PROGRAM instead of walking sched -> ElimStep ->
+// ElimNb -> ilist: one LduOp per elimination step with every offset and bound the three passes need already resolved.  A warp's ops
+// are contiguous and in phase order, so the address of the next op is a running index that does not wait on a load; the step count
+// of (phase, warp) is read next to it.  ElimStep and sched stay for the gradient pass.  Layout (ints, right after sched in the same
+// blob table): cnt[nphase][nw] steps of warp w in phase ph and wfirst[nw] first op of warp w from Plan::prog_cnt, padding to
+// 16 bytes, then LduOp ops[] from Plan::prog_ops.
+// An op is three 16-byte words of 16-bit arena offsets (an arena is < 2^16 doubles) and 8-bit sizes, so that the program costs the
+// hot prefix of the blob no table the chain kept in shared memory (quadruped's gradient pass has 9.2 KiB of room for it):
+//   word 0:  d_off | vec_off << 16,   n | nnb << 8 | fold_cnt << 16,   fold_off | fold[0] << 16,   fold[1] | fold[2] << 16
+//   word 1 + i, neighbour i:  L_off | fwd_abs << 16 (kLduNone: none),   vec_off | U_off << 16,   n | U_row << 8 | U_k << 16 | ld << 24,
+//                             tgt[i][0] | tgt[i][1] << 16
+// fold[] holds the first kLduFold scratch records folded into the step (arena offsets); the rest stay in Plan::ilist from fold_off.
+constexpr int kLduFold = 3;
+constexpr int kLduNone = 0xffff;
+struct alignas(16) LduOp {
+  int w[12];
+};
+static_assert(sizeof(LduOp) == 48, "LduOp is read as three 16-byte words");
+DJ_PLAN_FN int lo16(int v) { return v & 0xffff; }
+DJ_PLAN_FN int hi16(int v) { return (int)((unsigned)v >> 16); }
+DJ_PLAN_FN int byte_of(int v, int k) { return (v >> (8 * k)) & 0xff; }
+
 struct WarpRole {
   int npass;
   int type[3], first[3], count[3];
@@ -152,7 +174,8 @@ struct Plan {
   const JointDev* joints;
   const ContactDev* contacts;
   const ElimStep* steps;
-  const int* sched;   // [nphase][nw][2] = (first step, count)
+  const int* sched;   // [nphase][nw][2] = (first step, count), followed by the LDU program (LduOp)
+  int prog_cnt, prog_ops;  // ints from the start of sched to the program's cnt[] and ops[]
   const int* ilist;   // gather / fold lists
   const WarpRole* roles;  // [nw]
   // gradient pass

@@ -42,7 +42,7 @@ struct StepArgs {
   int slot_stride;      // doubles between the arenas of two slots of a CTA
   int T;                // time steps fused in this launch (rollouts: every environment is advanced T steps by one CTA)
   double* traj;         // nullable [T][B][nz]: state after every step
-  unsigned long long* prof;  // DJ_PROFILE builds: cycle counters [eval_jac, eval_ls, factorize, solve, misc]
+  unsigned long long* prof;  // DJ_PROFILE builds: cycle counters [eval_jac, eval_ls, factorize, solve, misc, ...] (layout: tools/time_variant.py)
   // Multi-GPU exchange fused into the step (SURVEY.md 8e, dojo_step_gather_async): besides Zn the epilogue writes every environment's
   // next state straight into the gathered buffer of every rank -- peer-mapped memory (CUDA IPC over NVLink / NVSwitch), this rank's
   // slice starts at gather_off doubles -- and every CTA signals the ranks when its share is out.  n_peers = 0: no exchange.
@@ -168,6 +168,7 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
 #ifdef DJ_PROFILE
   c.t_eval_jac = c.t_eval_ls = c.t_fact = c.t_solve = c.t_misc = c.t_align = c.t_cone = c.t_center = c.t_rolewait = 0; c.t_last = clock64();
   c.f_fold = c.f_inv = c.f_rm = c.f_schur = c.f_bar = 0;
+  c.s_cond = c.s_fwd = c.s_bwd = c.s_rec = c.s_bar = 0;
   long long k_c0 = clock64(); unsigned long long k_t0; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(k_t0));
   int k_envs = 0;
   if (c.tid == 0 && a.prof) atomicMin(a.prof + 31, k_t0);
@@ -330,6 +331,9 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
     atomicAdd(a.prof + 2, (unsigned long long)c.t_fact); atomicAdd(a.prof + 3, (unsigned long long)c.t_solve); atomicAdd(a.prof + 4, (unsigned long long)c.t_misc);
     atomicAdd(a.prof + 5, (unsigned long long)c.f_fold); atomicAdd(a.prof + 6, (unsigned long long)c.f_inv); atomicAdd(a.prof + 7, (unsigned long long)c.f_rm);
     atomicAdd(a.prof + 8, (unsigned long long)c.f_schur); atomicAdd(a.prof + 9, (unsigned long long)c.f_bar);
+    // solve(): 25 condense + gather, 26 forward sweep, 27 backward sweep, 28 recover, 29 slot barriers (17 + warp: role waits, nw <= 8)
+    atomicAdd(a.prof + 25, (unsigned long long)c.s_cond); atomicAdd(a.prof + 26, (unsigned long long)c.s_fwd); atomicAdd(a.prof + 27, (unsigned long long)c.s_bwd);
+    atomicAdd(a.prof + 28, (unsigned long long)c.s_rec); atomicAdd(a.prof + 29, (unsigned long long)c.s_bar);
     unsigned long long k_t1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(k_t1));
     atomicMax(a.prof + 10, (unsigned long long)(clock64() - k_c0)); atomicMax(a.prof + 11, k_t1 - k_t0);
     atomicMax(a.prof + 12, (unsigned long long)k_envs); atomicAdd(a.prof + 13, (unsigned long long)(clock64() - k_c0));

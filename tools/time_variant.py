@@ -43,4 +43,6 @@ if os.environ.get("DJ_PROF"):
     s.L.dojo_debug_cycles.argtypes = [C.c_void_p, C.c_void_p]
     s.L.dojo_debug_cycles(s.h, out)
     tot = sum(out)
-    print("   cycles/env-step: " + "  ".join(f"{n}={v/ (B*(20+steps)):.0f}" for n, v in zip(("eval_jac","eval_ls","fact","solve","misc","f_fold","f_inv","f_rm","f_schur","f_bar","-","-","-","-","align","cone","center","rolewait_w0","rolewait_w1"), out) if n != "-"))
+    names = ("eval_jac", "eval_ls", "fact", "solve", "misc", "f_fold", "f_inv", "f_rm", "f_schur", "f_bar", "-", "-", "-", "-", "align", "cone", "center",
+             "rolewait_w0", "rolewait_w1", "-", "-", "-", "-", "-", "-", "s_cond", "s_fwd", "s_bwd", "s_rec", "s_bar")
+    print("   cycles/env-step: " + "  ".join(f"{n}={v/ (B*(20+steps)):.0f}" for n, v in zip(names, out) if n != "-"))
