@@ -7,6 +7,7 @@ Python has no `!`, so `step!` is `step`):
     step!(mechanism, z, u; opts)          simulation/step.jl:11     step(mechanism, z, u, opts=None)
     simulate!(mechanism, steps, storage, control!; opts)            simulate(mechanism, steps, control=None, record=False, opts=None)
                                           simulation/simulate.jl:16
+    controller! reading get_minimal_state (examples/control)        simulate(..., control=LinearFeedback(K, x_ref, u_ref, K_i, xi))
     get_maximal_gradients!(mechanism, z, u; opts)                   get_maximal_gradients(mechanism, z, u, opts=None)
                                           gradients/state.jl:69
     get_contact_gradients(mechanism)      gradients/contact.jl:1    get_contact_gradients(mechanism, z, u, opts=None)
@@ -135,17 +136,46 @@ def step(mechanism: Mechanism, z, u, opts=None, literal_q1: bool = False, device
     return Zn, status, iters
 
 
+class LinearFeedback:
+    """A controller! that reads the minimal state at every step (get_minimal_state, examples/control) and applies the time-varying
+    affine law  u_t = u_ref - K (x_t - x_ref) - K_i xi_t,  xi_t = xi_{t-1} + h (x_t - x_ref)  (the integral is updated before use, as
+    pendulum_pid.jl does).  K, K_i [nu, 2nu], x_ref [2nu], u_ref [nu], each optionally per environment ([B, ...]) or per step and
+    environment ([steps, 1 or B, ...]); K_i None: no integral term.  simulate(..., control=LinearFeedback(...)) evaluates the law inside
+    the fused rollout on the device and updates `xi` ([2nu], or [B, 2nu]), so that a second call continues the integral.
+    Examples: pendulum_pid.jl is K = [Kp Kd], K_i = [Ki 0], x_ref = [pi/2, 0]; cartpole_lqr.jl is an LQR row on the cart input."""
+
+    def __init__(self, K, x_ref=None, u_ref=None, K_i=None, xi=None):
+        self.K, self.x_ref, self.u_ref, self.K_i = K, x_ref, u_ref, K_i
+        self.xi = None if xi is None else np.array(xi, dtype=float)
+
+
 def simulate(mechanism: Mechanism, steps: int, z0=None, control: Optional[Callable] = None, record: bool = False, opts=None, device: int = 0):
     """simulate!(mechanism, steps, storage, control!): `control(k)` returns the input(s) of step k ([nu] or [B, nu]; None = 0).
     Returns the final state(s) and, with record=True, the trajectory [steps, B, 13Nb] (the reference's Storage).
     The steps are fused into one launch, except with opts.verbose and a single environment: then every step is its own traced
-    launch and prints its solver table, as simulate! does with verbose = true (same results).  Batched calls do not print."""
+    launch and prints its solver table, as simulate! does with verbose = true (same results).  Batched calls do not print.
+    control = LinearFeedback(...) closes the loop on the device: the law is evaluated at every step on the state the step starts from,
+    in the same single launch (opts.verbose is refused: a traced closed loop is not provided)."""
     z0 = mechanism.z0 if z0 is None else z0
     z0 = np.asarray(z0, dtype=float)
     single = z0.ndim == 1
     Z = np.atleast_2d(z0)
     B = Z.shape[0]
     s = _stepper(mechanism, B, device)
+    if isinstance(control, LinearFeedback):
+        if _verbose(opts):
+            raise ValueError("simulate: opts.verbose with a LinearFeedback controller is not supported (the traced step runs open loop)")
+        fb = control
+        Zf, _, traj, _, xi = s.rollout_feedback(Z, steps, fb.K, fb.x_ref, fb.u_ref, fb.K_i, fb.xi, opts, record=record)
+        if xi is not None:
+            new = xi[0] if (single and (fb.xi is None or np.ndim(fb.xi) == 1)) else xi
+            if fb.xi is not None and np.shape(fb.xi) == new.shape:
+                fb.xi[...] = new
+            else:
+                fb.xi = new
+        if single:
+            return (Zf[0], traj[:, 0]) if record else Zf[0]
+        return (Zf, traj) if record else Zf
     U = None
     if control is not None:
         U = np.zeros((steps, B, mechanism.nu))
@@ -340,6 +370,8 @@ def simulate_record(mechanism: Mechanism, steps: int, z0=None, control: Optional
     z0 = mechanism.z0 if z0 is None else z0
     Z = np.atleast_2d(np.asarray(z0, dtype=float))
     B = Z.shape[0]
+    if isinstance(control, LinearFeedback):
+        raise ValueError("simulate_record: a LinearFeedback controller is not supported (use simulate(..., control=fb, record=True))")
     s = _stepper(mechanism, B, device)
     U = None
     if control is not None:

@@ -56,6 +56,12 @@ class DojoEnvSpec(C.Structure):
                 ("survive_reward", C.c_double), ("healthy_min", C.c_double), ("healthy_max", C.c_double), ("bound_abs", C.c_double)]
 
 
+class DojoFeedback(C.Structure):
+    """Closed-loop rollout law (include/dojo_b200.h: DojoFeedback): u_t = u_ref - K (x_t - x_ref) - K_i xi_t on the minimal state.
+    Every array holds steps (1 or T) x envs (1 or B) entries; K and K_i are column-major [nu x 2nu] per entry."""
+    _fields_ = [("steps", C.c_int32), ("envs", C.c_int32), ("K", c_double_p), ("K_i", c_double_p), ("x_ref", c_double_p), ("u_ref", c_double_p)]
+
+
 def env_spec(n_unactuated=0, contact_obs=False, forward_index=-1, healthy_index=-1, bound_index=-1, w_forward=0.0, w_control=0.0,
              w_contact=0.0, survive_reward=0.0, healthy_min=-float("inf"), healthy_max=float("inf"), bound_abs=float("inf")) -> DojoEnvSpec:
     return DojoEnvSpec(int(n_unactuated), int(bool(contact_obs)), int(forward_index), int(healthy_index), int(bound_index), float(w_forward),

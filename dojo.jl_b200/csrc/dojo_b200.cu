@@ -51,6 +51,13 @@ static const void* step_rec_kernel_fn(bool any_contact, bool plan_smem) {
   if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<false, true, false, false, true>;
   return (const void*)dojo_step_kernel<false, false, false, false, true>;
 }
+// the closed-loop rollout kernel (dojo_rollout_feedback) of the same compilation and plan placement; generic, like the REC kernel
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_fb_kernel();
+static const void* step_fb_kernel_fn(bool any_contact, bool plan_smem) {
+  if (any_contact) return dojo_cm_step_fb_kernel();
+  if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<false, true, false, false, false, true>;
+  return (const void*)dojo_step_kernel<false, false, false, false, false, true>;
+}
 
 // Order of the work queue.  A per-step launch ends when its slowest environment ends: an environment that stalls (ten line-search
 // trials per iteration up to max_iter, ~6 x the median time) and is dequeued late finishes alone.  Which environments stall is not
@@ -208,6 +215,11 @@ struct DojoHandle {
   size_t rpairs = 0;
   double *d_rZ = nullptr, *d_rU = nullptr, *d_rX = nullptr;
   size_t rZ_bytes = 0, rU_bytes = 0, rX_bytes = 0;
+  const void* k_fwd_fb = nullptr;                  // closed-loop rollout kernel (FB), set up by the first dojo_rollout_feedback call
+  int envs_per_sm_fb = 1;
+  double* d_fbX = nullptr;                         // FB scratch: x_t [2nu x max_batch], then u_t [nu x max_batch] (no U_applied)
+  double* d_fb = nullptr;                          // grow-only staging of host-pointer dojo_rollout_feedback calls
+  size_t fb_bytes = 0;
   std::string err;
 };
 // Whether the forward kernel specialised for small mechanisms (dojo_step_kernel.cuh, SMALL) computes this handle's step exactly: the
@@ -799,6 +811,7 @@ extern "C" int dojo_destroy(DojoHandle* h) {
   if (h->ev_last) cudaEventDestroy(h->ev_last);
   cudaFree(h->d_rollU); cudaFree(h->d_rollTraj);
   cudaFree(h->d_rsol); cudaFree(h->d_rdone); cudaFree(h->d_rstatus); cudaFree(h->d_riters); cudaFree(h->d_rZ); cudaFree(h->d_rU); cudaFree(h->d_rX);
+  cudaFree(h->d_fbX); cudaFree(h->d_fb);
   delete h;
   return DOJO_OK;
 }
@@ -1737,6 +1750,102 @@ extern "C" int dojo_rollout_minimal_gradients(DojoHandle* h, const DojoSolverOpt
     if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_riters, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   }
   leave_call(h, s);
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  return DOJO_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Closed-loop rollout: simulate! with a linear feedback controller! on the minimal state (include/dojo_b200.h)
+// ------------------------------------------------------------------------------------------------------------
+// The FB kernel evaluates the law inside the fused rollout, so that a closed loop costs one launch like dojo_rollout instead of three
+// launches per step (maximal_to_minimal, the law, dojo_step), each of which waits for its slowest environment.
+static int ensure_fb_kernel(DojoHandle* h) {
+  if (h->k_fwd_fb) return DOJO_OK;
+  const void* k = step_fb_kernel_fn(h->any_contact, h->plan_smem_mask == 0xff);
+  int occ = 1;
+  CUDA_TRY(h, max_shared_memory(k, h->device));
+  CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, 32 * h->nw * h->slots, h->smem_fwd));
+  h->envs_per_sm_fb = std::max(1, occ);
+  if (!h->d_fbX) CUDA_TRY(h, cudaMalloc((void**)&h->d_fbX, (size_t)h->max_batch * 3 * h->plan.nu * sizeof(double)));
+  h->k_fwd_fb = k;
+  return DOJO_OK;
+}
+
+// argument checks shared by both entries: no launch before every check has passed
+static int feedback_setup(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* xi, bool buffers, const char* who) {
+  if (!h) return DOJO_EINVAL;
+  if (B <= 0 || B > h->max_batch || T <= 0 || !buffers || !fb || !fb->K || (fb->steps != 1 && fb->steps != T) || (fb->envs != 1 && fb->envs != B) ||
+      (fb->K_i && !xi) || h->plan.nu == 0) {
+    h->err = std::string(who) + ": bad arguments (B in 1..max_batch, T >= 1, Z0 / Z_final / feedback / K required, steps in {1, T}, envs in {1, B}, "
+             "xi required with K_i, the mechanism must have inputs)";
+    return DOJO_EINVAL;
+  }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  return ensure_fb_kernel(h);
+}
+
+// fb's arrays are device pointers here
+static int launch_feedback(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const DojoFeedback* fb, double* dxi, double* dZf,
+                           double* dtraj, double* dUa, int32_t* dstatus, cudaStream_t s) {
+  StepArgs a = step_args(h, opts, B, false);
+  a.Z = dZ0; a.Zn = dZf; a.status = dstatus; a.T = T; a.traj = dtraj;
+  a.fb_K = fb->K; a.fb_Ki = fb->K_i; a.fb_xref = fb->x_ref; a.fb_uref = fb->u_ref; a.fb_steps = fb->steps; a.fb_envs = fb->envs;
+  a.fb_x = h->d_fbX; a.fb_xi = dxi;
+  a.fb_u = dUa ? dUa : h->d_fbX + (size_t)h->max_batch * 2 * h->plan.nu; a.fb_u_T = dUa ? 1 : 0;
+  enter_call(h, s);
+  CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
+  const int grid = std::min((B + h->slots - 1) / h->slots, h->sm_count * h->envs_per_sm_fb);
+  { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(h->k_fwd_fb, dim3(grid), dim3(32 * h->nw * h->slots), kargs, h->smem_fwd, s)); }
+  CUDA_TRY(h, cudaGetLastError());
+  h->launches += 1;
+  leave_call(h, s);
+  return DOJO_OK;
+}
+
+extern "C" int dojo_rollout_feedback_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const DojoFeedback* fb,
+                                           double* dxi, double* dZ_final, double* dZ_traj, double* dU_applied, int32_t* dstatus_any, void* cuda_stream) {
+  int rc = feedback_setup(h, B, T, fb, dxi, dZ0 && dZ_final, "dojo_rollout_feedback_async");
+  if (rc != DOJO_OK) return rc;
+  return launch_feedback(h, opts, B, T, dZ0, fb, dxi, dZ_final, dZ_traj, dU_applied, dstatus_any, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int dojo_rollout_feedback(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const DojoFeedback* fb, double* xi,
+                                     double* Z_final, double* Z_traj, double* U_applied, int32_t* status_any) {
+  int rc = feedback_setup(h, B, T, fb, xi, Z0 && Z_final, "dojo_rollout_feedback");
+  if (rc != DOJO_OK) return rc;
+  cudaStream_t s = h->stream;
+  if (is_device_ptr(Z0)) {
+    rc = launch_feedback(h, opts, B, T, Z0, fb, xi, Z_final, Z_traj, U_applied, status_any, s);
+    if (rc != DOJO_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    return DOJO_OK;
+  }
+  rc = ensure_staging(h);
+  if (rc != DOJO_OK) return rc;
+  // one grow-only buffer: [K | K_i | x_ref | u_ref | xi | U_applied | Z_traj], absent arrays take no space
+  const Plan& P = h->plan;
+  const size_t ne = (size_t)fb->steps * fb->envs, nx = 2 * (size_t)P.nu, nk = P.nu * nx * ne;
+  const size_t n[7] = {nk, fb->K_i ? nk : 0, fb->x_ref ? nx * ne : 0, fb->u_ref ? P.nu * ne : 0, xi ? nx * B : 0,
+                       U_applied ? (size_t)P.nu * B * T : 0, Z_traj ? (size_t)P.nz * B * T : 0};
+  const double* src[5] = {fb->K, fb->K_i, fb->x_ref, fb->u_ref, xi};
+  size_t off[8] = {0};
+  for (int k = 0; k < 7; ++k) off[k + 1] = off[k] + n[k];
+  rc = grow_buffer(h, (void**)&h->d_fb, &h->fb_bytes, off[7] * sizeof(double));
+  if (rc != DOJO_OK) return rc;
+  double* d[7];
+  for (int k = 0; k < 7; ++k) d[k] = n[k] ? h->d_fb + off[k] : nullptr;
+  const size_t zbytes = (size_t)B * P.nz * sizeof(double);
+  CUDA_TRY(h, cudaMemcpyAsync(h->d_Z, Z0, zbytes, cudaMemcpyHostToDevice, s));
+  for (int k = 0; k < 5; ++k)
+    if (n[k]) CUDA_TRY(h, cudaMemcpyAsync(d[k], src[k], n[k] * sizeof(double), cudaMemcpyHostToDevice, s));
+  const DojoFeedback dfb = {fb->steps, fb->envs, d[0], d[1], d[2], d[3]};
+  rc = launch_feedback(h, opts, B, T, h->d_Z, &dfb, d[4], h->d_Zn, d[6], d[5], h->d_status, s);
+  if (rc != DOJO_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(Z_final, h->d_Zn, zbytes, cudaMemcpyDeviceToHost, s));
+  if (n[4]) CUDA_TRY(h, cudaMemcpyAsync(xi, d[4], n[4] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (n[5]) CUDA_TRY(h, cudaMemcpyAsync(U_applied, d[5], n[5] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (n[6]) CUDA_TRY(h, cudaMemcpyAsync(Z_traj, d[6], n[6] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (status_any) CUDA_TRY(h, cudaMemcpyAsync(status_any, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(h, cudaStreamSynchronize(s));
   return DOJO_OK;
 }

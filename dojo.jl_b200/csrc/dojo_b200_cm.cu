@@ -28,3 +28,7 @@ extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_trace_
 extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_rec_kernel() {
   return (const void*)dj_cm::dojo_step_kernel<false, false, false, false, true>;
 }
+// the closed-loop rollout kernel of this compilation (dojo_rollout_feedback)
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_fb_kernel() {
+  return (const void*)dj_cm::dojo_step_kernel<false, false, false, false, false, true>;
+}

@@ -87,43 +87,47 @@ DJ_DEV void min_to_max_env(const KinArgs& a, int e) {
   min_to_max_one(a.joints, a.order, a.Ne, a.h, a.in + (size_t)e * 2 * a.nu, a.out + (size_t)e * 13 * a.Nb);
 }
 
+// one joint: maximal z [13 Nb] -> its slice of the minimal x [2 nu].  Reads only the joint's parent and child bodies, so the joints of
+// one environment may be mapped in any order or in parallel (one lane per joint: the feedback stage of dojo_step_kernel<..., FB>)
+DJ_DEV void max_to_min_joint(const JointDev& jd, double h, const double* z, double* x) {
+  const int nt = jd.nfree_t, nr = jd.nfree_r, nuj = nt + nr;
+  if (nuj == 0) return;
+  double* xm = x + 2 * jd.u_off;
+  const BodyState A = kin_load(z, jd.parent), Bc = kin_load(z, jd.child);
+  const Quat qoffi = qinv(Quat{jd.qoff[0], jd.qoff[1], jd.qoff[2], jd.qoff[3]});
+  // one step backward in time
+  const V3 xa1 = A.x - h * A.v, xb1 = Bc.x - h * Bc.v;
+  const Quat qa1 = next_orientation(A.q, -A.w, h), qb1 = next_orientation(Bc.q, -Bc.w, h);
+  const V3 et = tra_displacement(jd, A.x, A.q, Bc.x, Bc.q);
+  const V3 et1 = tra_displacement(jd, xa1, qa1, xb1, qb1);
+  const Quat q = qmul(qmul(qoffi, qinv(A.q)), Bc.q);
+  const Quat q1 = qmul(qmul(qoffi, qinv(qa1)), qb1);
+  const V3 th = rotation_vector(q);
+  const V3 dth = (1.0 / h) * rotation_vector(qmul(qinv(q1), q));
+  const V3 det = (1.0 / h) * (et - et1);
+  for (int i = 0; i < nt; ++i) {
+    const V3 ai = v3(jd.At[3 * i], jd.At[3 * i + 1], jd.At[3 * i + 2]);
+    xm[i] = dot(ai, et);
+    xm[nuj + i] = dot(ai, det);
+  }
+  for (int i = 0; i < nr; ++i) {
+    const V3 ai = v3(jd.Ar[3 * i], jd.Ar[3 * i + 1], jd.Ar[3 * i + 2]);
+    xm[nt + i] = dot(ai, th);
+    xm[nuj + nt + i] = dot(ai, dth);
+  }
+}
+
 // one environment: maximal z [13 Nb] -> minimal x [2 nu]
 DJ_DEV void max_to_min_one(const JointDev* joints, int Ne, double h, const double* z, double* x) {
-  for (int j = 0; j < Ne; ++j) {
-    const JointDev& jd = joints[j];
-    const int nt = jd.nfree_t, nr = jd.nfree_r, nuj = nt + nr;
-    if (nuj == 0) continue;
-    double* xm = x + 2 * jd.u_off;
-    const BodyState A = kin_load(z, jd.parent), Bc = kin_load(z, jd.child);
-    const Quat qoffi = qinv(Quat{jd.qoff[0], jd.qoff[1], jd.qoff[2], jd.qoff[3]});
-    // one step backward in time
-    const V3 xa1 = A.x - h * A.v, xb1 = Bc.x - h * Bc.v;
-    const Quat qa1 = next_orientation(A.q, -A.w, h), qb1 = next_orientation(Bc.q, -Bc.w, h);
-    const V3 et = tra_displacement(jd, A.x, A.q, Bc.x, Bc.q);
-    const V3 et1 = tra_displacement(jd, xa1, qa1, xb1, qb1);
-    const Quat q = qmul(qmul(qoffi, qinv(A.q)), Bc.q);
-    const Quat q1 = qmul(qmul(qoffi, qinv(qa1)), qb1);
-    const V3 th = rotation_vector(q);
-    const V3 dth = (1.0 / h) * rotation_vector(qmul(qinv(q1), q));
-    const V3 det = (1.0 / h) * (et - et1);
-    for (int i = 0; i < nt; ++i) {
-      const V3 ai = v3(jd.At[3 * i], jd.At[3 * i + 1], jd.At[3 * i + 2]);
-      xm[i] = dot(ai, et);
-      xm[nuj + i] = dot(ai, det);
-    }
-    for (int i = 0; i < nr; ++i) {
-      const V3 ai = v3(jd.Ar[3 * i], jd.Ar[3 * i + 1], jd.Ar[3 * i + 2]);
-      xm[nt + i] = dot(ai, th);
-      xm[nuj + nt + i] = dot(ai, dth);
-    }
-  }
+  for (int j = 0; j < Ne; ++j) max_to_min_joint(joints[j], h, z, x);
 }
 
 DJ_DEV void max_to_min_env(const KinArgs& a, int e) {
   max_to_min_one(a.joints, a.Ne, a.h, a.in + (size_t)e * 13 * a.Nb, a.out + (size_t)e * 2 * a.nu);
 }
 
-#ifdef __CUDACC__
+// the map kernels belong to the main compilation (dojo_b200.cu); dojo_b200_cm.cu includes this header for max_to_min_joint only
+#if defined(__CUDACC__) && !defined(DJ_ANY_CONTACT)
 __global__ void dojo_min_to_max_kernel(const KinArgs a) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e < a.B) min_to_max_env(a, e);

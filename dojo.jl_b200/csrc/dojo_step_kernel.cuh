@@ -9,6 +9,7 @@
 #pragma once
 #include "../../include/dojo_b200.h"
 #include "dojo_grad.cuh"
+#include "dojo_kin.cuh"
 
 namespace dj {
 
@@ -53,7 +54,52 @@ struct StepArgs {
   // traced step (TRACE kernels only, T = 1): [5 x max_iter x B], the rows of mehrotra<true> per environment (dojo_kernels.cuh).  Last
   // member, so that the parameter offsets of every other member, and with them the untraced kernels, do not depend on it.
   double* trace;
+  // feedback rollout (FB kernels only, dojo_rollout_feedback): before step t the slot maps the state to minimal coordinates x_t and
+  // evaluates u_t = u_ref - K (x_t - x_ref) - K_i xi_t, xi_t = xi_{t-1} + h (x_t - x_ref).  Every array holds fb_steps (1 or T) x
+  // fb_envs (1 or B) entries, entry (t, e) at index t * fb_envs + e; K / K_i [nu x 2nu] column-major per entry.  After trace, so that
+  // no other member moves.
+  const double* fb_K;
+  const double* fb_Ki;    // nullable: no integral term
+  const double* fb_xref;  // nullable: 0
+  const double* fb_uref;  // nullable: 0
+  int fb_steps, fb_envs;
+  double* fb_x;   // [2nu x B] scratch: x_t of the step the slot is about to solve (global memory, L1/L2-resident)
+  double* fb_xi;  // [2nu x B] integral state, updated in place (required iff fb_Ki)
+  double* fb_u;   // u_t, where prologue reads it: [nu x B x T] (fb_u_T = 1, the applied inputs) or [nu x B] scratch (fb_u_T = 0)
+  int fb_u_T;
 };
+
+// feedback stage of the FB kernel for environment e before step t from state z (global memory); returns where u_t was written.
+// Lanes: one per joint for the map (max_to_min_joint reads only the joint's parent and child), one per entry of xi, one per input.
+DJ_DEV const double* feedback(Ctx& c, const StepArgs& a, const double* z, int e, int t) {
+  const Plan& P = *c.P;
+  const int nu = P.nu, nx = 2 * nu;
+  double* x = a.fb_x + (size_t)e * nx;
+  for (int j = c.tid; j < P.Ne; j += c.nthreads) max_to_min_joint(c.joints[j], P.h, z, x);
+  __threadfence_block();
+  slot_sync(c);
+  const size_t q = (size_t)(a.fb_steps > 1 ? t : 0) * a.fb_envs + (a.fb_envs > 1 ? e : 0);
+  const double* xr = a.fb_xref ? a.fb_xref + q * nx : nullptr;
+  double* xi = a.fb_Ki ? a.fb_xi + (size_t)e * nx : nullptr;
+  if (xi) {  // the integral is updated before it is used (pendulum_pid.jl)
+    for (int k = c.tid; k < nx; k += c.nthreads) xi[k] += P.h * (xr ? x[k] - xr[k] : x[k]);
+    __threadfence_block();
+    slot_sync(c);
+  }
+  const double* K = a.fb_K + q * nu * nx;
+  const double* Ki = xi ? a.fb_Ki + q * nu * nx : nullptr;
+  double* u = a.fb_u + ((size_t)(a.fb_u_T ? t : 0) * a.B + e) * nu;
+  for (int i = c.tid; i < nu; i += c.nthreads) {
+    double s = 0.0;
+    for (int k = 0; k < nx; ++k) s += K[i + (size_t)nu * k] * (xr ? x[k] - xr[k] : x[k]);
+    if (Ki)
+      for (int k = 0; k < nx; ++k) s += Ki[i + (size_t)nu * k] * xi[k];
+    u[i] = (a.fb_uref ? a.fb_uref[q * nu + i] : 0.0) - s;
+  }
+  __threadfence_block();
+  slot_sync(c);
+  return u;
+}
 
 // epilogue: update_state! + get_next_state (bodies/set.jl:22-36, mechanism/get.jl:126-134).  The default output is the
 // mechanism's state after the step, (x3, v25, q3, w25); DOJO_FLAG_Q1_LITERAL_RETURN reproduces step!'s literal return
@@ -99,10 +145,14 @@ __device__ __forceinline__ unsigned long long k_t0g(unsigned long long* prof) { 
 // kernel needs at pair p = t * B + e -- the final solution in sol_raw [nres x B x T], status [B x T], iters [B x T] (nullable) -- and
 // publishes p on done_list (nullable).  a.traj is slab 1 of the [nz x B x (T + 1)] trajectory whose slab 0 is a.Z, so that pair p
 // starts from a.Z + p * nz; Zn is not written.  A compile-time parameter, so that the other instantiations are the same code as without it.
-template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false, bool SMALL = false, bool REC = false>
+// FB (forward, untraced, generic): the closed-loop rollout of dojo_rollout_feedback.  Before the prologue of step t the slot evaluates the
+// linear feedback law on the state the step starts from (feedback() above) and the step reads u_t from a.fb_u; a.U is not read.  The step
+// itself is dojo_rollout's.  A compile-time parameter, like REC.
+template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false, bool SMALL = false, bool REC = false, bool FB = false>
 __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(const StepArgs a) {
   static_assert(!SMALL || (!GRAD && PLAN_SMEM && !TRACE), "SMALL is a specialisation of the untraced forward kernel with the plan in shared memory");
   static_assert(!REC || (!GRAD && !TRACE && !SMALL), "REC is a variant of the generic untraced forward kernel");
+  static_assert(!FB || (!GRAD && !TRACE && !SMALL && !REC), "FB is a variant of the generic untraced forward kernel");
   extern __shared__ double arena[];
   __shared__ __align__(8) int s_env[128];  // CTA-wide mailbox, layout: dojo_kernels.cuh (cta_align)
   // a CTA hosts a.slots environments at a time; slot k is served by threads [k * 32 nw, (k + 1) * 32 nw)
@@ -201,6 +251,7 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
     if (!GRAD) {
       for (int t = 0; t < a.T; ++t) {
         const double* u = a.U ? a.U + ((size_t)t * a.B + e) * P.nu : nullptr;
+        if (FB) u = feedback(c, a, z, e, t);
         const double* fx = a.Fext ? a.Fext + (size_t)e * 6 * P.Nb : nullptr;
         prologue(c, z, u, fx, false);
         status = mehrotra<TRACE, SMALL>(c, a.opts, &iters, TRACE ? a.trace + (size_t)e * max(a.opts.max_iter, 0) * 5 : nullptr);

@@ -29,7 +29,7 @@ EXPORTS = ["dojo_default_options", "dojo_create", "dojo_destroy", "dojo_last_err
            "dojo_step_grad_contact_async", "dojo_step_record", "dojo_step_record_async", "dojo_simulate_record",
            "dojo_gather_create", "dojo_gather_export", "dojo_gather_connect", "dojo_gather_buffer", "dojo_gather_destroy", "dojo_step_gather_async",
            "dojo_step_grad_gather_async", "dojo_step_trace", "dojo_step_trace_async", "dojo_rollout_grad", "dojo_rollout_grad_async",
-           "dojo_rollout_minimal_gradients"]
+           "dojo_rollout_minimal_gradients", "dojo_rollout_feedback", "dojo_rollout_feedback_async"]
 
 _lib = None
 
@@ -124,6 +124,11 @@ def load_library():
     L.dojo_rollout_grad_async.restype = C.c_int
     L.dojo_rollout_minimal_gradients.argtypes = [vp, op, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
     L.dojo_rollout_minimal_gradients.restype = C.c_int
+    fp = C.POINTER(capi.DojoFeedback)
+    L.dojo_rollout_feedback.argtypes = [vp, op, C.c_int, C.c_int, vp, fp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_feedback.restype = C.c_int
+    L.dojo_rollout_feedback_async.argtypes = [vp, op, C.c_int, C.c_int, vp, fp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_feedback_async.restype = C.c_int
     L.dojo_gather_create.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
     L.dojo_gather_create.restype = C.c_int
     L.dojo_gather_export.argtypes = [vp, vp]
@@ -149,6 +154,28 @@ def _p(a):
     if isinstance(a, (int, np.integer)):
         return C.c_void_p(int(a))
     return C.c_void_p(a.ctypes.data)
+
+
+def feedback_arrays(T: int, B: int, nu: int, K, x_ref=None, u_ref=None, K_i=None):
+    """The arrays of a DojoFeedback from the shapes BatchedStepper.rollout_feedback accepts: a matrix (K, K_i) as [nu, 2nu], [B, nu, 2nu],
+    [T, 1, nu, 2nu] or [T, B, nu, 2nu], a vector (x_ref [2nu], u_ref [nu]) likewise.  All arrays share one (steps, envs): each is broadcast
+    to the largest given.  Returns (steps, envs, K, x_ref, u_ref, K_i) with every given array C-contiguous [steps, envs, ...] and the
+    matrices column-major per entry ([steps, envs, 2nu, nu]); absent arrays stay None."""
+    def lead(a, tail):
+        a = np.asarray(a, dtype=np.float64)
+        n = a.ndim - len(tail)
+        if a.shape[n:] != tail or n < 0 or n > 2 or (n == 1 and a.shape[0] != B) or (n == 2 and (a.shape[0] != T or a.shape[1] not in (1, B))):
+            raise ValueError(f"feedback array of shape {a.shape}: expected {tail}, (B,) + {tail} or (T, 1 or B) + {tail} with T = {T}, B = {B}")
+        return a.reshape(((1, 1), (1, B), a.shape[:2])[n] + tail)
+    shapes = {"K": (nu, 2 * nu), "x_ref": (2 * nu,), "u_ref": (nu,), "K_i": (nu, 2 * nu)}
+    given = {k: lead(v, shapes[k]) for k, v in (("K", K), ("x_ref", x_ref), ("u_ref", u_ref), ("K_i", K_i)) if v is not None}
+    steps = max(a.shape[0] for a in given.values())
+    envs = max(a.shape[1] for a in given.values())
+    out = {}
+    for k, a in given.items():
+        a = np.broadcast_to(a, (steps, envs) + shapes[k])
+        out[k] = np.ascontiguousarray(a.swapaxes(2, 3) if a.ndim == 4 else a)
+    return steps, envs, out["K"], out.get("x_ref"), out.get("u_ref"), out.get("K_i")
 
 
 class BatchedStepper:
@@ -339,6 +366,31 @@ class BatchedStepper:
         rc = self.L.dojo_rollout_minimal_gradients(self.h, C.byref(o), B, T, _p(X0), _p(U), _p(Xt), _p(Gx), _p(Gu), _p(status), _p(iters))
         self._check(rc, "dojo_rollout_minimal_gradients")
         return Xt, np.transpose(Gx, (0, 1, 3, 2)), np.transpose(Gu, (0, 1, 3, 2)), status, iters
+
+    def rollout_feedback(self, Z0, T: int, K, x_ref=None, u_ref=None, K_i=None, xi=None, opts=None, record: bool = False):
+        """Closed-loop rollout (dojo_rollout_feedback): before every step t the device maps the state to minimal coordinates x_t and applies
+        u_t = u_ref - K (x_t - x_ref) - K_i xi_t with xi_t = xi_{t-1} + h (x_t - x_ref), in the one launch of dojo_rollout.  K / K_i as
+        [nu, 2nu], [B, nu, 2nu], [T, 1, nu, 2nu] or [T, B, nu, 2nu], x_ref / u_ref likewise (feedback_arrays); xi [B, 2nu] or [2nu]
+        (zero when K_i is given without it).  Returns (Z_final [B, 13Nb], status_any [B], Z_traj [T, B, 13Nb] or None (record=False),
+        U_applied [T, B, nu], xi [B, 2nu] or None (no K_i)).  dojo_rollout(Z0, U_applied) reproduces the trajectory bit for bit."""
+        Z0 = np.ascontiguousarray(np.atleast_2d(Z0), dtype=np.float64)
+        B, T = Z0.shape[0], int(T)
+        assert Z0.shape[1] == self.nz
+        steps, envs, Kc, xr, ur, Kic = feedback_arrays(T, B, self.nu, K, x_ref, u_ref, K_i)
+        fb = capi.DojoFeedback(steps, envs, capi.dptr(Kc), None if Kic is None else capi.dptr(Kic), None if xr is None else capi.dptr(xr),
+                               None if ur is None else capi.dptr(ur))
+        if Kic is not None:
+            xi = np.zeros((B, 2 * self.nu)) if xi is None else np.array(np.broadcast_to(np.asarray(xi, dtype=np.float64), (B, 2 * self.nu)))
+        else:
+            xi = None
+        Zf = np.empty_like(Z0)
+        traj = np.empty((T, B, self.nz)) if record and T > 0 else None
+        Ua = np.empty((max(T, 0), B, self.nu))
+        st = np.zeros(B, dtype=np.int32)
+        o = opts if opts is not None else capi.solver_options()
+        rc = self.L.dojo_rollout_feedback(self.h, C.byref(o), B, T, _p(Z0), C.byref(fb), _p(xi), _p(Zf), _p(traj), _p(Ua), _p(st))
+        self._check(rc, "dojo_rollout_feedback")
+        return Zf, st, traj, Ua, xi
 
     # ------------------------------------------------------------------ minimal coordinates (SURVEY 8 f1)
     @property
@@ -573,6 +625,17 @@ class BatchedStepper:
         rc = self.L.dojo_rollout_grad_async(self.h, C.byref(o), int(B), int(T), _p(dZ0), _p(dU), _p(dZ_traj), _p(dFz), _p(dFu), _p(dstatus),
                                             _p(diters), C.c_void_p(int(stream)))
         self._check(rc, "dojo_rollout_grad_async")
+
+    def rollout_feedback_device(self, dZ0: int, dZf: int, B: int, T: int, dK: int, steps: int = 1, envs: int = 1, dK_i=None, dx_ref=None, du_ref=None,
+                                dxi=None, dtraj=None, dU_applied=None, dstatus=None, opts=None, stream: int = 0):
+        """dojo_rollout_feedback_async on device pointers: K / K_i [steps, envs, 2nu, nu] (column-major [nu x 2nu] per entry), x_ref
+        [steps, envs, 2nu], u_ref [steps, envs, nu], xi [B, 2nu] in/out, Z_traj [T, B, 13Nb], U_applied [T, B, nu], status [B]."""
+        o = opts if opts is not None else capi.solver_options()
+        cp = lambda d: None if d is None else C.cast(C.c_void_p(int(d)), capi.c_double_p)
+        fb = capi.DojoFeedback(int(steps), int(envs), cp(dK), cp(dK_i), cp(dx_ref), cp(du_ref))
+        rc = self.L.dojo_rollout_feedback_async(self.h, C.byref(o), int(B), int(T), _p(dZ0), C.byref(fb), _p(dxi), _p(dZf), _p(dtraj), _p(dU_applied),
+                                                _p(dstatus), C.c_void_p(int(stream)))
+        self._check(rc, "dojo_rollout_feedback_async")
 
     # ---- multi-GPU: the exchange of the next states fused into the step (include/dojo_b200.h, SURVEY.md 8e)
     def gather_create(self, world: int, rank: int, B_local: int):

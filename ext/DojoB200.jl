@@ -248,6 +248,37 @@ function rollout(mech::Mechanism, Z0::Matrix{Float64}, U::Array{Float64,3}; opts
     return Zf, traj
 end
 
+struct CFeedback  # = DojoFeedback (include/dojo_b200.h)
+    steps::Int32; envs::Int32
+    K::Ptr{Float64}; K_i::Ptr{Float64}; x_ref::Ptr{Float64}; u_ref::Ptr{Float64}
+end
+"closed-loop batched simulate! (examples/control: a controller! that reads get_minimal_state): before every step t the device applies
+ u_t = u_ref - K (x_t - x_ref) - K_i xi_t, xi_t = xi_{t-1} + h (x_t - x_ref), on the minimal state x_t, all T steps in one launch.
+ K, K_i: nu x 2nu, nu x 2nu x B or nu x 2nu x (1 or B) x T; x_ref (2nu) and u_ref (nu) likewise; every array is broadcast to the largest.
+ xi (2nu x B, zeros when K_i is given without it) is updated in place.  Returns (Z_final, Z_traj 13Nb x B x T or nothing,
+ U_applied nu x B x T, xi); rollout(mech, Z0, U_applied) reproduces the trajectory bit for bit"
+function rollout_feedback(mech::Mechanism, Z0::Matrix{Float64}, T::Integer, K::AbstractArray; x_ref = nothing, u_ref = nothing, K_i = nothing,
+                          xi = nothing, opts = SolverOptions{Float64}(), record = true)
+    h = handle(mech); B = size(Z0, 2); nu = h.nu
+    lay(A, tail) = A === nothing ? nothing : reshape(Float64.(A), tail..., size(A, length(tail) + 1), size(A, length(tail) + 2))
+    arrs = (lay(K, (nu, 2nu)), lay(K_i, (nu, 2nu)), lay(x_ref, (2nu,)), lay(u_ref, (nu,)))
+    given = [a for a in arrs if a !== nothing]
+    envs = maximum(size(a, ndims(a) - 1) for a in given); steps = maximum(size(a, ndims(a)) for a in given)
+    full(a) = a === nothing ? nothing : (o = zeros(size(a)[1:end-2]..., envs, steps); o .= a; o)
+    Kf, Kif, xrf, urf = map(full, arrs)
+    (Kif !== nothing && xi === nothing) && (xi = zeros(2nu, B))
+    p(a) = a === nothing ? Ptr{Float64}(C_NULL) : pointer(a)
+    Zf = similar(Z0); traj = record ? zeros(h.nz, B, T) : nothing; Ua = zeros(nu, B, T); status = zeros(Int32, B)
+    rc = GC.@preserve Kf Kif xrf urf begin
+        fb = CFeedback(Int32(steps), Int32(envs), p(Kf), p(Kif), p(xrf), p(urf))
+        ccall((:dojo_rollout_feedback, LIB), Cint,
+              (Ptr{Cvoid}, Ref{COptions}, Cint, Cint, Ptr{Float64}, Ref{CFeedback}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}),
+              h.ptr, COptions(opts), B, T, Z0, fb, xi === nothing ? C_NULL : xi, Zf, record ? traj : C_NULL, Ua, status)
+    end
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return Zf, traj, Ua, xi
+end
+
 "simulate! + get_maximal_gradients! at every step, fused: U is nu x B x T; returns (Z_traj 13Nb x B x (T+1) with Z_traj[:, :, 1] = Z0,
  Fz 12Nb x 12Nb x B x T, Fu 12Nb x nu x B x T, status B x T) -- Fz[:, :, e, t] = dz_{t+1}/dz_t"
 function rollout_gradients(mech::Mechanism, Z0::Matrix{Float64}, U::Array{Float64,3}; opts = SolverOptions{Float64}())

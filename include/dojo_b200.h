@@ -19,6 +19,8 @@
  *                                                                  src/gradients/state.jl:69-126
  *   dojo_rollout                 <- simulate!(mechanism, steps, storage, control!)
  *                                                                  src/simulation/simulate.jl:16-36
+ *   dojo_rollout_feedback        <- simulate!(mechanism, steps, storage, controller!) with a controller! that reads
+ *                                   get_minimal_state and applies a time-varying linear law (examples/control)
  *   dojo_rollout_grad            <- simulate! + get_maximal_gradients! at every step
  *   dojo_rollout_minimal_gradients <- simulate! + get_minimal_gradients! at every step
  *   DojoSolverOptions            <- SolverOptions{T}               src/solver/options.jl:16-26
@@ -280,6 +282,34 @@ int dojo_rollout(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, con
 int dojo_rollout_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0,
                        const double* dU, double* dZ_final, double* dZ_traj, int32_t* dstatus_any,
                        void* cuda_stream);
+
+/* Closed-loop rollout: simulate! with a controller! that reads the minimal state at every step and sets a time-varying affine
+ * law (examples/control: pendulum_pid.jl, cartpole_lqr.jl; the forward pass of iLQR / DDP / TVLQR).  In the ONE launch of
+ * dojo_rollout, before step t of every environment:
+ *   x_t  = maximal_to_minimal(z_t)                           (per joint [c_tra; c_rot; v_tra; v_rot], as dojo_maximal_to_minimal)
+ *   xi_t = xi_{t-1} + h (x_t - x_ref_t)                      (only with K_i; xi_{-1} = the caller's xi, updated before use)
+ *   u_t  = u_ref_t - K_t (x_t - x_ref_t) - K_i,t xi_t
+ *   z_{t+1} = step(z_t, u_t)                                 (dojo_rollout's step, bit for bit)
+ * Every array of DojoFeedback holds `steps` (1 or T) x `envs` (1 or B) entries, entry (t, e) at t * envs + e: one for all steps or
+ * one per step, one for all environments or one per environment.  K and K_i are column-major [nu x 2nu] per entry. */
+typedef struct {
+  int32_t steps, envs;   /* 1 or T / 1 or B */
+  const double* K;       /* [nu x 2nu x envs x steps], required */
+  const double* K_i;     /* same shape, nullable: no integral term */
+  const double* x_ref;   /* [2nu x envs x steps], nullable: 0 */
+  const double* u_ref;   /* [nu x envs x steps], nullable: 0 */
+} DojoFeedback;
+/* xi [2nu x B]: integral state, in/out (required iff K_i; after the call it holds xi_{T-1}, so that a second call continues it);
+ * Z_final [13Nb x B], Z_traj nullable [13Nb x B x T] and status_any [B] as dojo_rollout; U_applied nullable [nu x B x T]: u_t of every
+ * step -- dojo_rollout or dojo_rollout_grad driven by it reproduce the trajectory bit for bit.  Host or device pointers (all of one
+ * kind; host buffers are staged through grow-only handle buffers); *_async: device pointers, no synchronisation.
+ * DOJO_EINVAL, before anything is launched, unless B in 1..max_batch, T >= 1, fb and K given, steps in {1, T}, envs in {1, B},
+ * xi given with K_i, and nu > 0.  Flags, external forces and the Q1 literal return are single-step features. */
+int dojo_rollout_feedback(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const DojoFeedback* fb,
+                          double* xi, double* Z_final, double* Z_traj, double* U_applied, int32_t* status_any);
+int dojo_rollout_feedback_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const DojoFeedback* fb,
+                                double* dxi, double* dZ_final, double* dZ_traj, double* dU_applied, int32_t* dstatus_any,
+                                void* cuda_stream);
 
 /* Minimal <-> maximal coordinate maps (the step either side of step! for every DojoEnvironments call).
  * Minimal state x = per joint, in joint order, [c_tra; c_rot; v_tra; v_rot] (2 * input_dimension(joint) entries:
