@@ -22,6 +22,7 @@ Python has no `!`, so `step!` is `step`):
     minimal_to_maximal_jacobian(mechanism, x)  gradients/state.jl:136 minimal_to_maximal_jacobian(mechanism, x)
     get_minimal_gradients!(mechanism, x, u; opts)                   get_minimal_gradients(mechanism, x, u, opts=None)
                                           gradients/state.jl:182
+    IterativeLQR.jl (docs/src/examples/trajectory_optimization.md)  ilqr(mechanism, x0, U0, QuadraticCost(Q, R, ...), iterations)
     simulate!(...; record=true) -> Storage  simulation/simulate.jl:16, storage.jl:15-67      simulate_record(mechanism, steps, ...) -> Storage
     momentum / kinetic_energy / potential_energy / mechanical_energy(mechanism, storage)   same names (mechanics/{momentum,energy}.jl)
 
@@ -45,7 +46,7 @@ import numpy as np
 
 from . import capi
 from .mechanism import Mechanism
-from .solver import DOJO_FLAG_Q1_LITERAL_RETURN, DOJO_FLAG_Q2_LITERAL_GRADIENTS, STATUS, BatchedStepper
+from .solver import DOJO_FLAG_Q1_LITERAL_RETURN, DOJO_FLAG_Q2_LITERAL_GRADIENTS, STATUS, BatchedStepper, cost_arrays
 
 SolverOptions = capi.solver_options
 
@@ -327,6 +328,100 @@ def get_minimal_gradients(mechanism: Mechanism, x, u, opts=None, device: int = 0
         _check_single(status)
         return Gx[0], Gu[0]
     return Gx, Gu
+
+
+class QuadraticCost:
+    """The quadratic tracking cost of trajectory optimisation in minimal coordinates (dojo_lqr_backward's DojoQuadraticCost):
+        J = sum_t 1/2 (x_t - xg_t)' Q_t (x_t - xg_t) + 1/2 (u_t - ug_t)' R_t (u_t - ug_t)  +  1/2 (x_T - xg_T)' Q_final (x_T - xg_T).
+    Q [2nu, 2nu], R [nu, nu], x_goal [2nu], u_goal [nu], each also per environment [B, ...] or per step [T, 1 or B, ...]; Q_final and
+    x_goal_final also [B, ...].  Defaults: goals 0, Q_final = the last step's Q, x_goal_final = the last step's x_goal."""
+
+    def __init__(self, Q, R, x_goal=None, u_goal=None, Q_final=None, x_goal_final=None):
+        self.Q, self.R, self.x_goal, self.u_goal, self.Q_final, self.x_goal_final = Q, R, x_goal, u_goal, Q_final, x_goal_final
+
+    def evaluate(self, X_traj, U):
+        """J per environment [B] of X_traj [T+1, B, 2nu] and U [T, B, nu] (None: 0)"""
+        X_traj = np.asarray(X_traj, dtype=float)
+        T, B, nx = X_traj.shape[0] - 1, X_traj.shape[1], X_traj.shape[2]
+        _, _, Q, R, xg, ug, Qf, xgf = cost_arrays(T, B, nx // 2, self.Q, self.R, self.x_goal, self.u_goal, self.Q_final, self.x_goal_final)
+        dx = X_traj[:T] - (0.0 if xg is None else xg)
+        du = (0.0 if U is None else np.asarray(U, dtype=float)) - (0.0 if ug is None else ug)
+        du = np.broadcast_to(du, (T, B, nx // 2))
+        # the arrays are column-major per entry: Q[t, e, j, i] = Q_t[i, j]
+        J = 0.5 * np.einsum("tbi,tbji,tbj->b", dx, np.broadcast_to(Q, (T, B, nx, nx)), dx)
+        J += 0.5 * np.einsum("tbi,tbji,tbj->b", du, np.broadcast_to(R, (T, B) + R.shape[2:]), du)
+        dxf = X_traj[T] - (0.0 if xgf is None else xgf)
+        return J + 0.5 * np.einsum("bi,bji,bj->b", dxf, np.broadcast_to(Qf, (B, nx, nx)), dxf)
+
+
+def ilqr(mechanism: Mechanism, x0, U0, cost: QuadraticCost, iterations: int = 20, active=None, opts=None, device: int = 0, mu0: float = 0.0,
+         tol: float = 1e-10):
+    """iLQR in minimal coordinates for a batch of B problems, as IterativeLQR.jl runs Dojo's examples (trajectory_optimization.md),
+    without constraints.  x0 [B, 2nu] or [2nu], U0 [T, nu] or [T, B, nu] the initial inputs, cost a QuadraticCost, active [nu] mask of
+    the inputs the optimiser may change (None: all; the others stay at U0).  Every iteration is three device calls:
+      1. rollout_minimal_gradients(x0, U): the nominal X and the Jacobians Gx, Gu;
+      2. lqr_backward: the gains K, k and the expected decrease dV; where its Cholesky fails, mu is raised for that environment and the
+         pass repeated;
+      3. a backtracking line search per environment, alpha = 1, 1/2, ..., 1/512: rollout_feedback(K, x_ref = X, u_ref = U + alpha k)
+         is accepted when the cost decreases by at least 1e-4 (alpha dV1 + alpha^2 dV2) in magnitude.  The accepted U_applied is the
+         next nominal, so the next rollout reproduces the accepted trajectory bit for bit.  Where no trial is accepted, mu is raised and
+         the trajectory kept; an environment whose expected decrease falls below tol (1 + J) has converged and keeps its trajectory.
+    Returns (X [T+1, B, 2nu], U [T, B, nu], K [T, B, nu, 2nu], k [T, B, nu] (the gains of a final backward pass about X, U), J
+    [iterations+1, B] (the cost before each iteration and at the end; non-increasing), status [B]: 0 converged, 1 not converged within
+    `iterations`, 2 the backward pass or the line search failed at the largest regularisation (1e8))."""
+    x0 = np.asarray(x0, dtype=float)
+    X0 = np.atleast_2d(x0)
+    B, nu = X0.shape[0], mechanism.nu
+    U0 = np.asarray(U0, dtype=float)
+    T = U0.shape[0]
+    U = np.ascontiguousarray(np.broadcast_to(U0.reshape(T, -1, nu), (T, B, nu)))
+    s = _stepper(mechanism, B, device)
+    Z0 = s.minimal_to_maximal(X0)
+    mu = np.full(B, float(mu0))
+    status = np.ones(B, dtype=np.int32)
+    hist = []
+
+    def backward(X, U, Gx, Gu):
+        K, k, dV, st = s.lqr_backward(X, U, Gx, Gu, cost, mu, active)
+        while (st != 0).any() and (mu[st != 0] < 1e8).any():
+            mu[st != 0] = np.maximum(10.0 * mu[st != 0], 1e-6)
+            K, k, dV, st = s.lqr_backward(X, U, Gx, Gu, cost, mu, active)
+        return K, k, dV, st
+
+    X, Gx, Gu, _, _ = s.rollout_minimal_gradients(X0, U, T, opts)
+    J = cost.evaluate(X, U)
+    for _ in range(iterations):
+        hist.append(J)
+        K, k, dV, st = backward(X, U, Gx, Gu)
+        active_env = (status == 1) & (st == 0)
+        status[(status == 1) & (st != 0)] = 2
+        converged = active_env & (-(dV[:, 0] + dV[:, 1]) <= tol * (1.0 + np.abs(J)))
+        status[converged] = 0
+        pending = active_env & ~converged
+        if not pending.any():
+            break
+        K, k = np.nan_to_num(K), np.nan_to_num(k)
+        Un = U.copy()
+        for alpha in 0.5 ** np.arange(10):
+            _, _, traj, Ua, _ = s.rollout_feedback(Z0, T, K, x_ref=X[:T], u_ref=U + alpha * k, opts=opts, record=True)
+            Xt = np.stack([X[0]] + [s.maximal_to_minimal(traj[t]) for t in range(T)])
+            Jt = cost.evaluate(Xt, Ua)
+            ok = pending & np.isfinite(Jt) & (Jt <= J) & (J - Jt >= -1e-4 * (alpha * dV[:, 0] + alpha ** 2 * dV[:, 1]))
+            Un[:, ok] = Ua[:, ok]
+            pending &= ~ok
+            if not pending.any():
+                break
+        mu[pending] = np.maximum(10.0 * mu[pending], 1e-6)
+        status[pending & (mu > 1e8)] = 2
+        accepted = active_env & ~converged & ~pending
+        mu[accepted] = np.where(mu[accepted] > 1e-6, 0.1 * mu[accepted], mu0)
+        U = Un
+        X, Gx, Gu, _, _ = s.rollout_minimal_gradients(X0, U, T, opts)
+        J = cost.evaluate(X, U)
+    while len(hist) < iterations + 1:
+        hist.append(J)
+    K, k, _, _ = s.lqr_backward(X, U, Gx, Gu, cost, mu, active)
+    return X, U, K, k, np.array(hist), status
 
 
 class Storage:

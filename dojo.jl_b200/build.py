@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdojo_b200.so")
 SOURCES = ["dojo_b200.cu", "dojo_b200_cm.cu"]
-HEADERS = ["dojo_step_kernel.cuh", "dojo_contact_orthant.cuh", "dojo_joint_tra.cuh", "dojo_kernels.cuh", "dojo_grad.cuh", "dojo_kin.cuh", "dojo_kinjac.cuh", "dojo_envs.cuh", "dojo_storage.cuh", "dojo_linalg.cuh", "dojo_math.cuh", "dojo_plan.h", os.path.join("..", "..", "include", "dojo_b200.h")]
+HEADERS = ["dojo_step_kernel.cuh", "dojo_contact_orthant.cuh", "dojo_joint_tra.cuh", "dojo_kernels.cuh", "dojo_grad.cuh", "dojo_kin.cuh", "dojo_kinjac.cuh", "dojo_envs.cuh", "dojo_storage.cuh", "dojo_lqr.cuh", "dojo_linalg.cuh", "dojo_math.cuh", "dojo_plan.h", os.path.join("..", "..", "include", "dojo_b200.h")]
 
 
 def nvcc_path() -> str:

@@ -62,6 +62,19 @@ class DojoFeedback(C.Structure):
     _fields_ = [("steps", C.c_int32), ("envs", C.c_int32), ("K", c_double_p), ("K_i", c_double_p), ("x_ref", c_double_p), ("u_ref", c_double_p)]
 
 
+class DojoQuadraticCost(C.Structure):
+    """Quadratic tracking cost of dojo_lqr_backward (include/dojo_b200.h: DojoQuadraticCost).  Q, R, x_goal, u_goal hold steps (1 or T) x
+    envs (1 or B) entries, Q_final and x_goal_final envs entries; matrices column-major per entry."""
+    _fields_ = [("steps", C.c_int32), ("envs", C.c_int32), ("Q", c_double_p), ("R", c_double_p), ("x_goal", c_double_p), ("u_goal", c_double_p),
+                ("Q_final", c_double_p), ("x_goal_final", c_double_p)]
+
+
+def quadratic_cost(steps, envs, Q, R, x_goal=None, u_goal=None, Q_final=None, x_goal_final=None) -> DojoQuadraticCost:
+    """a DojoQuadraticCost over host arrays (solver.cost_arrays's output); the arrays must outlive the struct"""
+    p = lambda a: None if a is None else dptr(a)
+    return DojoQuadraticCost(int(steps), int(envs), p(Q), p(R), p(x_goal), p(u_goal), p(Q_final), p(x_goal_final))
+
+
 def env_spec(n_unactuated=0, contact_obs=False, forward_index=-1, healthy_index=-1, bound_index=-1, w_forward=0.0, w_control=0.0,
              w_contact=0.0, survive_reward=0.0, healthy_min=-float("inf"), healthy_max=float("inf"), bound_abs=float("inf")) -> DojoEnvSpec:
     return DojoEnvSpec(int(n_unactuated), int(bool(contact_obs)), int(forward_index), int(healthy_index), int(bound_index), float(w_forward),

@@ -18,6 +18,7 @@
 #include "dojo_kinjac.cuh"
 #include "dojo_envs.cuh"
 #include "dojo_storage.cuh"
+#include "dojo_lqr.cuh"
 
 using namespace dj;
 
@@ -220,6 +221,9 @@ struct DojoHandle {
   double* d_fbX = nullptr;                         // FB scratch: x_t [2nu x max_batch], then u_t [nu x max_batch] (no U_applied)
   double* d_fb = nullptr;                          // grow-only staging of host-pointer dojo_rollout_feedback calls
   size_t fb_bytes = 0;
+  double* d_lqr = nullptr;                         // grow-only staging of host-pointer dojo_lqr_backward calls
+  size_t lqr_bytes = 0;
+  bool lqr_ready = false;                          // dojo_lqr_backward_kernel has the device's shared-memory maximum
   std::string err;
 };
 // Whether the forward kernel specialised for small mechanisms (dojo_step_kernel.cuh, SMALL) computes this handle's step exactly: the
@@ -811,7 +815,7 @@ extern "C" int dojo_destroy(DojoHandle* h) {
   if (h->ev_last) cudaEventDestroy(h->ev_last);
   cudaFree(h->d_rollU); cudaFree(h->d_rollTraj);
   cudaFree(h->d_rsol); cudaFree(h->d_rdone); cudaFree(h->d_rstatus); cudaFree(h->d_riters); cudaFree(h->d_rZ); cudaFree(h->d_rU); cudaFree(h->d_rX);
-  cudaFree(h->d_fbX); cudaFree(h->d_fb);
+  cudaFree(h->d_fbX); cudaFree(h->d_fb); cudaFree(h->d_lqr);
   delete h;
   return DOJO_OK;
 }
@@ -1846,6 +1850,105 @@ extern "C" int dojo_rollout_feedback(DojoHandle* h, const DojoSolverOptions* opt
   if (n[5]) CUDA_TRY(h, cudaMemcpyAsync(U_applied, d[5], n[5] * sizeof(double), cudaMemcpyDeviceToHost, s));
   if (n[6]) CUDA_TRY(h, cudaMemcpyAsync(Z_traj, d[6], n[6] * sizeof(double), cudaMemcpyDeviceToHost, s));
   if (status_any) CUDA_TRY(h, cudaMemcpyAsync(status_any, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  return DOJO_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Riccati backward pass of iLQR / TVLQR in minimal coordinates (include/dojo_b200.h, dojo_lqr.cuh)
+// ------------------------------------------------------------------------------------------------------------
+// threads per CTA (one CTA per environment): enough 2 x 2 tiles of the nx x nx products per thread to hide shared-memory latency
+static int lqr_threads(int nu) { return nu <= 4 ? 64 : nu <= 16 ? 128 : nu <= 24 ? 256 : 512; }
+
+// argument checks shared by both entries (no launch before every check has passed); fills the kernel arguments but the arrays
+static int lqr_setup(DojoHandle* h, int B, int T, const DojoQuadraticCost* c, const int32_t* active, bool buffers, LqrArgs* a, const char* who) {
+  if (!h) return DOJO_EINVAL;
+  const int nu = h->plan.nu;
+  int na = 0;
+  if (active)
+    for (int i = 0; i < nu; ++i) na += active[i] != 0;
+  if (B <= 0 || B > h->max_batch || T <= 0 || !buffers || !c || !c->Q || !c->R || !c->Q_final || (c->steps != 1 && c->steps != T) ||
+      (c->envs != 1 && c->envs != B) || nu == 0 || (active && na == 0)) {
+    h->err = std::string(who) + ": bad arguments (B in 1..max_batch, T >= 1, cost / Q / R / Q_final / X_traj / Gx / Gu / K / k required, "
+             "steps in {1, T}, envs in {1, B}, the mechanism must have inputs, `active` must have a nonzero entry)";
+    return DOJO_EINVAL;
+  }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  int optin = 0;
+  CUDA_TRY(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+  if (nu > DJ_LQR_MAX_NU || lqr_smem_bytes(nu) > (size_t)optin) {
+    h->err = std::string(who) + ": the Riccati working set of one environment (" + std::to_string(lqr_smem_bytes(nu)) +
+             " bytes) exceeds the shared memory of one block";
+    return DOJO_ENOMEM;
+  }
+  if (!h->lqr_ready) {
+    CUDA_TRY(h, max_shared_memory((const void*)dojo_lqr_backward_kernel, h->device));
+    h->lqr_ready = true;
+  }
+  *a = LqrArgs{};
+  a->nu = nu; a->B = B; a->T = T; a->steps = c->steps; a->envs = c->envs;
+  for (int i = 0; i < nu; ++i)
+    if (!active || active[i]) a->act[a->na++] = i;
+  return DOJO_OK;
+}
+
+static int launch_lqr(DojoHandle* h, const LqrArgs& a, cudaStream_t s) {
+  enter_call(h, s);
+  void* kargs[1] = {(void*)&a};
+  CUDA_TRY(h, cudaLaunchKernel((const void*)dojo_lqr_backward_kernel, dim3(a.B), dim3(lqr_threads(a.nu)), kargs, lqr_smem_bytes(a.nu), s));
+  CUDA_TRY(h, cudaGetLastError());
+  h->launches += 1;
+  leave_call(h, s);
+  return DOJO_OK;
+}
+
+extern "C" int dojo_lqr_backward_async(DojoHandle* h, int B, int T, const DojoQuadraticCost* cost, const int32_t* active, const double* dX_traj,
+                                       const double* dU, const double* dGx, const double* dGu, const double* dmu, double* dK, double* dk, double* ddV,
+                                       int32_t* dstatus, void* cuda_stream) {
+  LqrArgs a;
+  int rc = lqr_setup(h, B, T, cost, active, dX_traj && dGx && dGu && dK && dk, &a, "dojo_lqr_backward_async");
+  if (rc != DOJO_OK) return rc;
+  a.Q = cost->Q; a.R = cost->R; a.xg = cost->x_goal; a.ug = cost->u_goal; a.Qf = cost->Q_final; a.xgf = cost->x_goal_final;
+  a.X = dX_traj; a.U = dU; a.Gx = dGx; a.Gu = dGu; a.mu = dmu; a.K = dK; a.k = dk; a.dV = ddV; a.status = dstatus;
+  return launch_lqr(h, a, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int dojo_lqr_backward(DojoHandle* h, int B, int T, const DojoQuadraticCost* cost, const int32_t* active, const double* X_traj,
+                                 const double* U, const double* Gx, const double* Gu, const double* mu, double* K, double* k, double* dV,
+                                 int32_t* status) {
+  LqrArgs a;
+  int rc = lqr_setup(h, B, T, cost, active, X_traj && Gx && Gu && K && k, &a, "dojo_lqr_backward");
+  if (rc != DOJO_OK) return rc;
+  cudaStream_t s = h->stream;
+  if (is_device_ptr(X_traj)) {
+    rc = dojo_lqr_backward_async(h, B, T, cost, active, X_traj, U, Gx, Gu, mu, K, k, dV, status, s);
+    if (rc != DOJO_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    return DOJO_OK;
+  }
+  // one grow-only buffer: [Q | R | x_goal | u_goal | Q_final | x_goal_final | X_traj | U | Gx | Gu | mu | K | k | dV | status],
+  // absent arrays take no space
+  const size_t nu = a.nu, nx = 2 * nu, ne = (size_t)cost->steps * cost->envs, pairs = (size_t)B * T;
+  const size_t n[15] = {nx * nx * ne, nu * nu * ne, cost->x_goal ? nx * ne : 0, cost->u_goal ? nu * ne : 0, nx * nx * cost->envs,
+                        cost->x_goal_final ? nx * cost->envs : 0, nx * (pairs + B), U ? nu * pairs : 0, nx * nx * pairs, nx * nu * pairs,
+                        mu ? (size_t)B : 0, nu * nx * pairs, nu * pairs, dV ? 2 * (size_t)B : 0, status ? ((size_t)B + 1) / 2 : 0};
+  const double* src[11] = {cost->Q, cost->R, cost->x_goal, cost->u_goal, cost->Q_final, cost->x_goal_final, X_traj, U, Gx, Gu, mu};
+  size_t off[16] = {0};
+  for (int i = 0; i < 15; ++i) off[i + 1] = off[i] + n[i];
+  rc = grow_buffer(h, (void**)&h->d_lqr, &h->lqr_bytes, off[15] * sizeof(double));
+  if (rc != DOJO_OK) return rc;
+  double* d[15];
+  for (int i = 0; i < 15; ++i) d[i] = n[i] ? h->d_lqr + off[i] : nullptr;
+  for (int i = 0; i < 11; ++i)
+    if (n[i]) CUDA_TRY(h, cudaMemcpyAsync(d[i], src[i], n[i] * sizeof(double), cudaMemcpyHostToDevice, s));
+  a.Q = d[0]; a.R = d[1]; a.xg = d[2]; a.ug = d[3]; a.Qf = d[4]; a.xgf = d[5];
+  a.X = d[6]; a.U = d[7]; a.Gx = d[8]; a.Gu = d[9]; a.mu = d[10]; a.K = d[11]; a.k = d[12]; a.dV = d[13]; a.status = (int32_t*)d[14];
+  rc = launch_lqr(h, a, s);
+  if (rc != DOJO_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(K, d[11], n[11] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(k, d[12], n[12] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (dV) CUDA_TRY(h, cudaMemcpyAsync(dV, d[13], n[13] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, d[14], (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(h, cudaStreamSynchronize(s));
   return DOJO_OK;
 }

@@ -29,7 +29,7 @@ EXPORTS = ["dojo_default_options", "dojo_create", "dojo_destroy", "dojo_last_err
            "dojo_step_grad_contact_async", "dojo_step_record", "dojo_step_record_async", "dojo_simulate_record",
            "dojo_gather_create", "dojo_gather_export", "dojo_gather_connect", "dojo_gather_buffer", "dojo_gather_destroy", "dojo_step_gather_async",
            "dojo_step_grad_gather_async", "dojo_step_trace", "dojo_step_trace_async", "dojo_rollout_grad", "dojo_rollout_grad_async",
-           "dojo_rollout_minimal_gradients", "dojo_rollout_feedback", "dojo_rollout_feedback_async"]
+           "dojo_rollout_minimal_gradients", "dojo_rollout_feedback", "dojo_rollout_feedback_async", "dojo_lqr_backward", "dojo_lqr_backward_async"]
 
 _lib = None
 
@@ -129,6 +129,11 @@ def load_library():
     L.dojo_rollout_feedback.restype = C.c_int
     L.dojo_rollout_feedback_async.argtypes = [vp, op, C.c_int, C.c_int, vp, fp, vp, vp, vp, vp, vp, vp]
     L.dojo_rollout_feedback_async.restype = C.c_int
+    cp = C.POINTER(capi.DojoQuadraticCost)
+    L.dojo_lqr_backward.argtypes = [vp, C.c_int, C.c_int, cp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_lqr_backward.restype = C.c_int
+    L.dojo_lqr_backward_async.argtypes = [vp, C.c_int, C.c_int, cp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_lqr_backward_async.restype = C.c_int
     L.dojo_gather_create.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
     L.dojo_gather_create.restype = C.c_int
     L.dojo_gather_export.argtypes = [vp, vp]
@@ -156,26 +161,60 @@ def _p(a):
     return C.c_void_p(a.ctypes.data)
 
 
+def _entries(T: int, B: int, arrays: dict, what: str):
+    """Broadcast {name: (array or None, tail shape)} to one (steps, envs): each array is given as tail, (B,) + tail or (T, 1 or B) + tail
+    and is broadcast to the largest given.  Returns (steps, envs, {name: C-contiguous [steps, envs] + tail, matrices column-major per
+    entry}) for the given arrays."""
+    def lead(a, tail):
+        a = np.asarray(a, dtype=np.float64)
+        n = a.ndim - len(tail)
+        if a.shape[n:] != tail or n < 0 or n > 2 or (n == 1 and a.shape[0] != B) or (n == 2 and (a.shape[0] != T or a.shape[1] not in (1, B))):
+            raise ValueError(f"{what} array of shape {a.shape}: expected {tail}, (B,) + {tail} or (T, 1 or B) + {tail} with T = {T}, B = {B}")
+        return a.reshape(((1, 1), (1, B), a.shape[:2])[n] + tail)
+    given = {k: (lead(v, tail), tail) for k, (v, tail) in arrays.items() if v is not None}
+    steps = max(a.shape[0] for a, _ in given.values())
+    envs = max(a.shape[1] for a, _ in given.values())
+    out = {}
+    for k, (a, tail) in given.items():
+        a = np.broadcast_to(a, (steps, envs) + tail)
+        out[k] = np.ascontiguousarray(a.swapaxes(2, 3) if a.ndim == 4 else a)
+    return steps, envs, out
+
+
 def feedback_arrays(T: int, B: int, nu: int, K, x_ref=None, u_ref=None, K_i=None):
     """The arrays of a DojoFeedback from the shapes BatchedStepper.rollout_feedback accepts: a matrix (K, K_i) as [nu, 2nu], [B, nu, 2nu],
     [T, 1, nu, 2nu] or [T, B, nu, 2nu], a vector (x_ref [2nu], u_ref [nu]) likewise.  All arrays share one (steps, envs): each is broadcast
     to the largest given.  Returns (steps, envs, K, x_ref, u_ref, K_i) with every given array C-contiguous [steps, envs, ...] and the
     matrices column-major per entry ([steps, envs, 2nu, nu]); absent arrays stay None."""
-    def lead(a, tail):
-        a = np.asarray(a, dtype=np.float64)
-        n = a.ndim - len(tail)
-        if a.shape[n:] != tail or n < 0 or n > 2 or (n == 1 and a.shape[0] != B) or (n == 2 and (a.shape[0] != T or a.shape[1] not in (1, B))):
-            raise ValueError(f"feedback array of shape {a.shape}: expected {tail}, (B,) + {tail} or (T, 1 or B) + {tail} with T = {T}, B = {B}")
-        return a.reshape(((1, 1), (1, B), a.shape[:2])[n] + tail)
-    shapes = {"K": (nu, 2 * nu), "x_ref": (2 * nu,), "u_ref": (nu,), "K_i": (nu, 2 * nu)}
-    given = {k: lead(v, shapes[k]) for k, v in (("K", K), ("x_ref", x_ref), ("u_ref", u_ref), ("K_i", K_i)) if v is not None}
-    steps = max(a.shape[0] for a in given.values())
-    envs = max(a.shape[1] for a in given.values())
-    out = {}
-    for k, a in given.items():
-        a = np.broadcast_to(a, (steps, envs) + shapes[k])
-        out[k] = np.ascontiguousarray(a.swapaxes(2, 3) if a.ndim == 4 else a)
+    steps, envs, out = _entries(T, B, {"K": (K, (nu, 2 * nu)), "x_ref": (x_ref, (2 * nu,)), "u_ref": (u_ref, (nu,)), "K_i": (K_i, (nu, 2 * nu))},
+                                "feedback")
     return steps, envs, out["K"], out.get("x_ref"), out.get("u_ref"), out.get("K_i")
+
+
+def cost_arrays(T: int, B: int, nu: int, Q, R, x_goal=None, u_goal=None, Q_final=None, x_goal_final=None):
+    """The arrays of a DojoQuadraticCost, with the broadcasting rules of feedback_arrays: Q [2nu, 2nu], R [nu, nu], x_goal [2nu] and
+    u_goal [nu], each also per environment ([B, ...]) or per step ([T, 1 or B, ...]), broadcast to one (steps, envs); Q_final [2nu, 2nu]
+    and x_goal_final [2nu], each also [B, ...], broadcast to envs.  Q_final defaults to the last step's Q and x_goal_final to the last
+    step's x_goal.  Returns (steps, envs, Q, R, x_goal, u_goal, Q_final, x_goal_final), C-contiguous, Q / R as [steps, envs, n, n] and
+    Q_final as [envs, 2nu, 2nu] column-major per entry (Q, R, Q_final symmetric in use); absent goals stay None."""
+    nx = 2 * nu
+    steps, envs, out = _entries(T, B, {"Q": (Q, (nx, nx)), "R": (R, (nu, nu)), "x_goal": (x_goal, (nx,)), "u_goal": (u_goal, (nu,))}, "cost")
+    fin = {}
+    for k, a, tail in (("Q_final", Q_final, (nx, nx)), ("x_goal_final", x_goal_final, (nx,))):
+        if a is not None:
+            a = np.asarray(a, dtype=np.float64)
+            if a.shape not in (tail, (B,) + tail):
+                raise ValueError(f"final cost array of shape {a.shape}: expected {tail} or (B,) + {tail} with B = {B}")
+            fin[k] = a.reshape((1,) + tail if a.ndim == len(tail) else a.shape)
+    if any(a.shape[0] > envs for a in fin.values()):  # a per-environment final cost makes the running cost per environment too
+        envs = B
+        out = {k: np.ascontiguousarray(np.broadcast_to(a, (steps, envs) + a.shape[2:])) for k, a in out.items()}
+    for k, a in fin.items():
+        a = np.broadcast_to(a, (envs,) + a.shape[1:])
+        fin[k] = np.ascontiguousarray(a.swapaxes(1, 2) if a.ndim == 3 else a)
+    Qf = fin.get("Q_final", out["Q"][-1])
+    xgf = fin.get("x_goal_final", None if x_goal is None else out["x_goal"][-1])
+    return steps, envs, out["Q"], out["R"], out.get("x_goal"), out.get("u_goal"), Qf, xgf
 
 
 class BatchedStepper:
@@ -391,6 +430,31 @@ class BatchedStepper:
         rc = self.L.dojo_rollout_feedback(self.h, C.byref(o), B, T, _p(Z0), C.byref(fb), _p(xi), _p(Zf), _p(traj), _p(Ua), _p(st))
         self._check(rc, "dojo_rollout_feedback")
         return Zf, st, traj, Ua, xi
+
+    def lqr_backward(self, X_traj, U, Gx, Gu, cost, mu=None, active=None):
+        """Riccati backward pass of iLQR / TVLQR (dojo_lqr_backward) on the shapes rollout_minimal_gradients returns: X_traj [T+1, B, 2nu],
+        U [T, B, nu] or None, Gx [T, B, 2nu, 2nu], Gu [T, B, 2nu, nu].  cost has the attributes Q, R, x_goal, u_goal, Q_final,
+        x_goal_final (api.QuadraticCost; shapes as cost_arrays).  mu [B] or a scalar (None: 0); active [nu] mask (None: all inputs).
+        Returns (K [T, B, nu, 2nu], k [T, B, nu], dV [B, 2], status [B]): the law u = u_bar + alpha k - K (x - x_bar), the expected
+        decrease alpha dV[0] + alpha^2 dV[1], and per environment 0 or t + 1 when the Cholesky of Quu + mu I failed at step t (then its
+        K[:t+1], k[:t+1] and dV are NaN)."""
+        X_traj = np.ascontiguousarray(X_traj, dtype=np.float64)
+        T, B, nx = X_traj.shape[0] - 1, X_traj.shape[1], 2 * self.nu
+        assert X_traj.shape[2] == nx and T >= 1
+        Gx, Gu = np.asarray(Gx, dtype=np.float64), np.asarray(Gu, dtype=np.float64)
+        assert Gx.shape == (T, B, nx, nx) and Gu.shape == (T, B, nx, self.nu)
+        Gxc, Guc = np.ascontiguousarray(Gx.swapaxes(2, 3)), np.ascontiguousarray(Gu.swapaxes(2, 3))  # column-major per pair
+        if U is not None:
+            U = np.ascontiguousarray(U, dtype=np.float64)
+            assert U.shape == (T, B, self.nu)
+        ca = cost_arrays(T, B, self.nu, cost.Q, cost.R, cost.x_goal, cost.u_goal, cost.Q_final, cost.x_goal_final)
+        c = capi.quadratic_cost(*ca)
+        mu = None if mu is None else np.ascontiguousarray(np.broadcast_to(np.asarray(mu, dtype=np.float64), (B,)))
+        act = None if active is None else np.ascontiguousarray(np.asarray(active).astype(np.int32).reshape(self.nu))
+        K, k, dV, st = np.empty((T, B, nx, self.nu)), np.empty((T, B, self.nu)), np.empty((B, 2)), np.zeros(B, dtype=np.int32)
+        rc = self.L.dojo_lqr_backward(self.h, B, T, C.byref(c), _p(act), _p(X_traj), _p(U), _p(Gxc), _p(Guc), _p(mu), _p(K), _p(k), _p(dV), _p(st))
+        self._check(rc, "dojo_lqr_backward")
+        return np.transpose(K, (0, 1, 3, 2)), k, dV, st
 
     # ------------------------------------------------------------------ minimal coordinates (SURVEY 8 f1)
     @property
@@ -636,6 +700,19 @@ class BatchedStepper:
         rc = self.L.dojo_rollout_feedback_async(self.h, C.byref(o), int(B), int(T), _p(dZ0), C.byref(fb), _p(dxi), _p(dZf), _p(dtraj), _p(dU_applied),
                                                 _p(dstatus), C.c_void_p(int(stream)))
         self._check(rc, "dojo_rollout_feedback_async")
+
+    def lqr_backward_device(self, B: int, T: int, dX_traj: int, dGx: int, dGu: int, dK: int, dk: int, dQ: int, dR: int, dQ_final: int,
+                            steps: int = 1, envs: int = 1, dx_goal=None, du_goal=None, dx_goal_final=None, dU=None, dmu=None, active=None,
+                            ddV=None, dstatus=None, stream: int = 0):
+        """dojo_lqr_backward_async on device pointers, in the layouts of dojo_rollout_minimal_gradients: X_traj [T+1, B, 2nu], Gx / Gu
+        column-major per pair ([T, B, 2nu, 2nu] / [T, B, nu, 2nu] in memory), K out [T, B, 2nu, nu] in memory (column-major [nu x 2nu]),
+        k [T, B, nu], dV [B, 2], status [B]; the cost arrays as cost_arrays returns them; active: a host [nu] mask or None."""
+        cp = lambda d: None if d is None else C.cast(C.c_void_p(int(d)), capi.c_double_p)
+        c = capi.DojoQuadraticCost(int(steps), int(envs), cp(dQ), cp(dR), cp(dx_goal), cp(du_goal), cp(dQ_final), cp(dx_goal_final))
+        act = None if active is None else np.ascontiguousarray(np.asarray(active).astype(np.int32).reshape(self.nu))
+        rc = self.L.dojo_lqr_backward_async(self.h, int(B), int(T), C.byref(c), _p(act), _p(dX_traj), _p(dU), _p(dGx), _p(dGu), _p(dmu), _p(dK),
+                                            _p(dk), _p(ddV), _p(dstatus), C.c_void_p(int(stream)))
+        self._check(rc, "dojo_lqr_backward_async")
 
     # ---- multi-GPU: the exchange of the next states fused into the step (include/dojo_b200.h, SURVEY.md 8e)
     def gather_create(self, world: int, rank: int, B_local: int):

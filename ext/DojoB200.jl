@@ -301,6 +301,44 @@ function rollout_minimal_gradients(mech::Mechanism, X0::Matrix{Float64}, U::Arra
     return Xt, Gx, Gu, status
 end
 
+struct CQuadraticCost  # = DojoQuadraticCost (include/dojo_b200.h)
+    steps::Int32; envs::Int32
+    Q::Ptr{Float64}; R::Ptr{Float64}; x_goal::Ptr{Float64}; u_goal::Ptr{Float64}; Q_final::Ptr{Float64}; x_goal_final::Ptr{Float64}
+end
+"Riccati backward pass of iLQR / TVLQR (the backward pass of IterativeLQR.jl's solve!) on rollout_minimal_gradients' output, all
+ environments and steps in one launch: Xt 2nu x B x (T+1), U nu x B x T (or nothing), Gx 2nu x 2nu x B x T, Gu 2nu x nu x B x T.
+ Cost sum_t 1/2 |x_t - x_goal|^2_Q + 1/2 |u_t - u_goal|^2_R + 1/2 |x_T - x_goal_final|^2_Q_final: Q, R, x_goal, u_goal as nxn, nxnxB or
+ nxnx(1 or B)xT (broadcast to the largest, as rollout_feedback's arrays); Q_final (default: Q's last step) and x_goal_final (default:
+ x_goal's last step) n x n or n x n x B.  active: nu mask (nothing: all inputs), mu: B regularisations.  Returns (K nu x 2nu x B x T,
+ k nu x B x T, dV 2 x B, status B): u = U + alpha k - K (x - Xt) is rollout_feedback(mech, Z0, T, K; x_ref = Xt[:, :, 1:T],
+ u_ref = U + alpha k); status[e] = t when the Cholesky of Quu + mu I failed at step t (1-based; K, k up to it and dV are NaN)"
+function lqr_backward(mech::Mechanism, Xt::Array{Float64,3}, U, Gx::Array{Float64,4}, Gu::Array{Float64,4}; Q, R, x_goal = nothing,
+                      u_goal = nothing, Q_final = nothing, x_goal_final = nothing, active = nothing, mu = nothing)
+    h = handle(mech); B = size(Xt, 2); T = size(Xt, 3) - 1; nu = h.nu
+    lay(A, tail) = A === nothing ? nothing : reshape(Float64.(A), tail..., size(A, length(tail) + 1), size(A, length(tail) + 2))
+    arrs = (lay(Q, (2nu, 2nu)), lay(R, (nu, nu)), lay(x_goal, (2nu,)), lay(u_goal, (nu,)))
+    given = [a for a in arrs if a !== nothing]
+    fin = (Q_final === nothing ? nothing : reshape(Float64.(Q_final), 2nu, 2nu, :), x_goal_final === nothing ? nothing : reshape(Float64.(x_goal_final), 2nu, :))
+    envs = max(maximum(size(a, ndims(a) - 1) for a in given), maximum((size(a, ndims(a)) for a in fin if a !== nothing); init = 1))
+    steps = maximum(size(a, ndims(a)) for a in given)
+    full(a) = a === nothing ? nothing : (o = zeros(size(a)[1:end-2]..., envs, steps); o .= a; o)
+    Qs, Rs, xgs, ugs = map(full, arrs)
+    Qf = fin[1] === nothing ? Qs[:, :, :, end] : (o = zeros(2nu, 2nu, envs); o .= fin[1]; o)
+    xgf = fin[2] === nothing ? (xgs === nothing ? nothing : xgs[:, :, end]) : (o = zeros(2nu, envs); o .= fin[2]; o)
+    act = active === nothing ? C_NULL : Int32.(collect(active))
+    K = zeros(nu, 2nu, B, T); k = zeros(nu, B, T); dV = zeros(2, B); status = zeros(Int32, B)
+    p(a) = a === nothing ? Ptr{Float64}(C_NULL) : pointer(a)
+    rc = GC.@preserve Qs Rs xgs ugs Qf xgf begin
+        cost = CQuadraticCost(Int32(steps), Int32(envs), p(Qs), p(Rs), p(xgs), p(ugs), p(Qf), p(xgf))
+        ccall((:dojo_lqr_backward, LIB), Cint,
+              (Ptr{Cvoid}, Cint, Cint, Ref{CQuadraticCost}, Ptr{Int32}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+               Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}),
+              h.ptr, B, T, cost, act, Xt, U === nothing ? C_NULL : U, Gx, Gu, mu === nothing ? C_NULL : Float64.(mu), K, k, dV, status)
+    end
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return K, k, dV, status
+end
+
 # ---- multi-GPU: one Julia process per GPU (e.g. MPI.jl ranks or Distributed workers); the exchange of the next states is fused into
 # the step kernel (peer writes over NVLink, include/dojo_b200.h "Multi-GPU"): no NCCL.jl needed.  `allgather_bytes` is any host-side
 # all-gather of a 128-byte blob per rank (MPI.Allgather, a shared file, ...), used ONCE at set-up.

@@ -23,6 +23,9 @@
  *                                   get_minimal_state and applies a time-varying linear law (examples/control)
  *   dojo_rollout_grad            <- simulate! + get_maximal_gradients! at every step
  *   dojo_rollout_minimal_gradients <- simulate! + get_minimal_gradients! at every step
+ *   dojo_lqr_backward            <- the backward pass of IterativeLQR.jl's solve! (iLQR / TVLQR gains
+ *                                   from the minimal-coordinate Jacobians and a quadratic cost;
+ *                                   docs/src/examples/trajectory_optimization.md)
  *   DojoSolverOptions            <- SolverOptions{T}               src/solver/options.jl:16-26
  *   dojo_minimal_to_maximal      <- minimal_to_maximal(mechanism, x) src/mechanism/state.jl:9-22
  *                                   (set_minimal_coordinates_velocities!, src/joints/minimal.jl:148-203)
@@ -310,6 +313,43 @@ int dojo_rollout_feedback(DojoHandle* h, const DojoSolverOptions* opts, int B, i
 int dojo_rollout_feedback_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const DojoFeedback* fb,
                                 double* dxi, double* dZ_final, double* dZ_traj, double* dU_applied, int32_t* dstatus_any,
                                 void* cuda_stream);
+
+/* Riccati backward pass of time-varying LQR / iLQR in minimal coordinates, batched: one launch for all B environments and T steps.
+ * Cost per environment:  sum_t 1/2 (x_t - xg_t)' Q_t (x_t - xg_t) + 1/2 (u_t - ug_t)' R_t (u_t - ug_t)  +  1/2 (x_T - xg_T)' Q_f (x_T - xg_T).
+ * From the nominal trajectory (X_traj, U) and its Jacobians A_t = Gx[t, e], B_t = Gu[t, e] (the layouts dojo_rollout_minimal_gradients
+ * writes), for t = T-1 ... 0 with P_T = Q_f, p_T = Q_f (x_T - xg_T):
+ *   Qx = Q_t dx_t + A'p   Qu = R_t du_t + B'p   Qxx = Q_t + A'PA   Quu = R_t + B'PB   Qux = B'PA   (dx = x_t - xg_t, du = u_t - ug_t)
+ *   K_t = (Quu + mu_e I)^-1 Qux,   k_t = -(Quu + mu_e I)^-1 Qu          (Cholesky; on the active inputs only)
+ *   P = Qxx + K'Quu K - K'Qux - Qux'K (symmetrised),   p = Qx - K'Quu k - K'Qu + Qux'k,   dV += [k'Qu, 1/2 k'Quu k]
+ * (the P, p and dV updates use Quu without mu, as Tassa, Erez and Todorov 2012).  The forward law is u = u_bar + alpha k - K (x - x_bar):
+ * DojoFeedback with K, x_ref = X_traj, u_ref = U + alpha k, so K goes to dojo_rollout_feedback unchanged.
+ * Every array of DojoQuadraticCost holds `steps` (1 or T) x `envs` (1 or B) entries, entry (t, e) at t * envs + e, as DojoFeedback;
+ * Q_final and x_goal_final hold `envs` entries.  Matrices are column-major. */
+typedef struct {
+  int32_t steps, envs;          /* 1 or T / 1 or B */
+  const double* Q;              /* [2nu x 2nu x envs x steps], required */
+  const double* R;              /* [nu x nu x envs x steps], required */
+  const double* x_goal;         /* [2nu x envs x steps], nullable: 0 */
+  const double* u_goal;         /* [nu x envs x steps], nullable: 0 */
+  const double* Q_final;        /* [2nu x 2nu x envs], required */
+  const double* x_goal_final;   /* [2nu x envs], nullable: 0 */
+} DojoQuadraticCost;
+/* active [nu] (HOST array, nullable = all active): inputs with active = 0 (a floating base, an unactuated joint) get a zero row in K and
+ * a zero k, and Quu is factored on the active inputs only.  X_traj [2nu x B x (T+1)], U [nu x B x T] (nullable: 0), Gx [2nu x 2nu x B x T],
+ * Gu [2nu x nu x B x T], pair (t, e) at t * B + e.  mu [B] nullable: 0.  Outputs K [nu x 2nu x B x T] (= DojoFeedback.K with
+ * envs = B, steps = T), k [nu x B x T], dV [2 x B] nullable (the expected decrease alpha dV[0] + alpha^2 dV[1]), status [B] nullable:
+ * 0, or t + 1 when the Cholesky of Quu + mu I failed at step t -- then that environment's K_s and k_s for s <= t and its dV are NaN,
+ * and every other environment is unaffected.  Raise mu for it and call again.
+ * Host or device pointers (all of one kind; host buffers are staged through grow-only handle buffers); *_async: device pointers, no
+ * synchronisation.  DOJO_EINVAL, before anything is launched, unless B in 1..max_batch, T >= 1, cost / Q / R / Q_final / X_traj / Gx /
+ * Gu / K / k given, steps in {1, T}, envs in {1, B}, nu > 0 and `active`, if given, has a nonzero entry.  DOJO_ENOMEM when the working
+ * set of one environment (about 19 nu^2 doubles) exceeds the device's shared memory per block (nu <= 38 on H100). */
+int dojo_lqr_backward(DojoHandle* h, int B, int T, const DojoQuadraticCost* cost, const int32_t* active, const double* X_traj,
+                      const double* U, const double* Gx, const double* Gu, const double* mu, double* K, double* k, double* dV,
+                      int32_t* status);
+int dojo_lqr_backward_async(DojoHandle* h, int B, int T, const DojoQuadraticCost* cost, const int32_t* active, const double* dX_traj,
+                            const double* dU, const double* dGx, const double* dGu, const double* dmu, double* dK, double* dk, double* ddV,
+                            int32_t* dstatus, void* cuda_stream);
 
 /* Minimal <-> maximal coordinate maps (the step either side of step! for every DojoEnvironments call).
  * Minimal state x = per joint, in joint order, [c_tra; c_rot; v_tra; v_rot] (2 * input_dimension(joint) entries:
