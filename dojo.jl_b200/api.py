@@ -46,7 +46,7 @@ import numpy as np
 
 from . import capi
 from .mechanism import Mechanism
-from .solver import DOJO_FLAG_Q1_LITERAL_RETURN, DOJO_FLAG_Q2_LITERAL_GRADIENTS, STATUS, BatchedStepper, cost_arrays
+from .solver import DOJO_FLAG_Q1_LITERAL_RETURN, DOJO_FLAG_Q2_LITERAL_GRADIENTS, DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN, STATUS, BatchedStepper, cost_arrays
 
 SolverOptions = capi.solver_options
 
@@ -200,17 +200,19 @@ def simulate(mechanism: Mechanism, steps: int, z0=None, control: Optional[Callab
     return (Zf, traj) if record else Zf
 
 
-def get_maximal_gradients(mechanism: Mechanism, z, u, opts=None, device: int = 0, literal_q2: bool = False):
+def get_maximal_gradients(mechanism: Mechanism, z, u, opts=None, device: int = 0, literal_q2: bool = False, literal_q17: bool = False):
     """get_maximal_gradients!(mechanism, z, u; opts) -> (jacobian_state [12Nb x 12Nb], jacobian_control [12Nb x nu]);
     batched inputs give [B, 12Nb, 12Nb] and [B, 12Nb, nu].  literal_q2=True reproduces the reference's literal result (data
     Jacobian and chain rule at the state shifted by update_state!, gradients/state.jl:69-76); the default is the consistent
-    implicit-function-theorem gradient."""
+    implicit-function-theorem gradient.  literal_q17=True leaves d(input impulse)/d(configuration) out of the data Jacobian, as
+    gradients/data.jl does; the reference's get_maximal_gradients! is literal_q2=literal_q17=True."""
     z = np.asarray(z, dtype=float)
     single = z.ndim == 1
     Z = np.atleast_2d(z)
     U = np.atleast_2d(np.asarray(u, dtype=float))
     s = _stepper(mechanism, Z.shape[0], device)
-    _, Fz, Fu, status, _ = s.step_grad(Z, U, opts, flags=DOJO_FLAG_Q2_LITERAL_GRADIENTS if literal_q2 else 0)
+    flags = (DOJO_FLAG_Q2_LITERAL_GRADIENTS if literal_q2 else 0) | (DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN if literal_q17 else 0)
+    _, Fz, Fu, status, _ = s.step_grad(Z, U, opts, flags=flags)
     if single:
         _check_single(status)
         return Fz[0], Fu[0]

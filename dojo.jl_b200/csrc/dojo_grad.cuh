@@ -18,8 +18,9 @@
 // Everything is in attitude (body-frame) form: a perturbation q (x) (1, d).  The reference's attjac'd 6x6 blocks
 // (joints/*/impulses.jl impulse_transform_jacobian, springs.jl / dampers.jl *_jacobian_configuration, contacts/contact.jl
 // impulse_map_jacobian, integrators/integrator.jl integrator_jacobian_configuration) are re-derived in closed form.
-// As in the reference, d(input impulse)/d(configuration) is NOT part of the data Jacobian (gradients/data.jl has no
-// such term; test/data.jl runs with zero inputs).
+// Unlike the reference, the data Jacobian includes d(input impulse)/d(configuration) (SURVEY.md Q17: gradients/data.jl never
+// calls input_jacobian_configuration, so its Fz is not the derivative of the step once an actuated joint has a free parent and
+// u != 0).  DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN leaves the term out: gradients() is then called without the inputs.
 #pragma once
 #include "dojo_kernels.cuh"
 
@@ -296,7 +297,8 @@ DJ_DEV V3 grad_joint_tra(Ctx& c, const JointDev& jd, const Kin& ka, const Kin& k
 
 // record layout of a joint (doubles): RJp[nq*6] RJc[nq*6] BPp[36] BPc[36] BCp[36] BCc[36] Up[6*nu] Uc[6*nu]   (nq = joint_nq: the
 // node's rows = ne equality rows + one kept limit dual per limited axis)
-DJ_DEV void grad_joint(Ctx& c, int idx) {
+// u: this environment's inputs, or null to leave the inputs' configuration derivative out (SURVEY.md Q17)
+DJ_DEV void grad_joint(Ctx& c, int idx, const double* __restrict__ u) {
   const Plan& P = *c.P;
   double* A = c.A;
   const JointDev& jd = c.joints[idx];
@@ -354,18 +356,32 @@ DJ_DEV void grad_joint(Ctx& c, int idx) {
   if (jd.flags) pt += grad_joint_tra(c, jd, ka, kb, g2, g3, Ma, Mb, so, BPp, BPc, BCp, BCc, RJp, RJc);
 #endif
   // translational impulses (translational/impulses.jl:9-45):  F_p = -Ra p, F_c = Ra p, tau_p = p x (e + pa), tau_c = pb x (Rb' Ra p)
+  // The translational input it (prologue_joint) is such an impulse with only half of its torque (Q16): p = pt + it on the force
+  // rows, pt + it / 2 on the torque rows.
   {
+    V3 pf = pt, pq = pt;
+    if (u && jd.nfree_t > 0) {
+      V3 it = v3zero();
+#pragma unroll
+      for (int i = 0; i < 3; ++i)
+        if (i < jd.nfree_t) it += u[jd.u_off + i] * ld3(jd.At + 3 * i);
+      it = P.input_scaling * it;
+      pf = pt + it;
+      pq = pt + 0.5 * it;
+    }
     V3 pb = ld3(jd.pb);
-    M33 Rasp = Ra * skew(pt);
+    M33 Rasp = Ra * skew(pf);
     add_block33(BPp, 6, 0, 3, Rasp, 2.0);    // dF_p / d phi_a
     add_block33(BCp, 6, 0, 3, Rasp, -2.0);   // dF_c / d phi_a
-    M33 sp = skew(pt);
+    M33 sp = skew(pq);
     add_block33(BPp, 6, 3, 0, sp * g2.Xp); add_block33(BPp, 6, 3, 3, sp * g2.Qtp);
     add_block33(BPc, 6, 3, 0, sp * g2.Xc); add_block33(BPc, 6, 3, 3, sp * g2.Qtc);
     M33 RbtRa = transpose(Rb) * Ra;
     add_block33(BCp, 6, 3, 3, skew(pb) * (RbtRa * sp), -2.0);
-    add_block33(BCc, 6, 3, 3, skew(pb) * skew(RbtRa * pt), 2.0);
+    add_block33(BCc, 6, 3, 3, skew(pb) * skew(RbtRa * pq), 2.0);
   }
+  Quat r = qmul(qinv(ka.q2), kb.q2);
+  M33 Rr = rotmat(r), Rrt = transpose(Rr);
   // rotational impulses (rotational/impulses.jl:9-38): tau_c = 1/2 (s p - v x p), tau_p = -1/2 Roff (s p + v x p)
   {
     M33 sp = skew(pr);
@@ -374,12 +390,20 @@ DJ_DEV void grad_joint(Ctx& c, int idx) {
     M33 dc_a = 0.5 * (outer(pr, Rv) + sp * g2.Qrp);        // d tau_c / d phi_a
     M33 dp_b = (-0.5) * (Roff * (outer(pr, -vr) - sp * g2.Qrc));
     M33 dp_a = (-0.5) * (Roff * (outer(pr, Rv) - sp * g2.Qrp));
+    // rotational input (rotational/input.jl:5-17): tau_p = -Roff tau is constant, tau_c = -R(r)' tau_p turns with r
+    if (u && jd.nfree_r > 0) {
+      V3 ir = v3zero();
+#pragma unroll
+      for (int i = 0; i < 3; ++i)
+        if (i < jd.nfree_r) ir += u[jd.u_off + jd.nfree_t + i] * ld3(jd.Ar + 3 * i);
+      V3 tp = (-P.input_scaling) * (Roff * ir);
+      dc_a = dc_a + 2.0 * (Rrt * skew(tp));
+      dc_b = dc_b + (-2.0) * skew(Rrt * tp);
+    }
     add_block33(BCc, 6, 3, 3, dc_b); add_block33(BCp, 6, 3, 3, dc_a);
     add_block33(BPc, 6, 3, 3, dp_b); add_block33(BPp, 6, 3, 3, dp_a);
     (void)s0;
   }
-  Quat r = qmul(qinv(ka.q2), kb.q2);
-  M33 Rr = rotmat(r), Rrt = transpose(Rr);
   M33 AtA = m33zero();
 #pragma unroll
   for (int i = 0; i < 3; ++i)
@@ -684,7 +708,8 @@ DJ_DEV void grad_write_column(Ctx& c, const double* V, int ch, int col, int lane
 
 // the whole gradient pass for one environment; the KKT blocks of the final iterate must be assembled (unfactorised)
 // Fc (nullable): [12 Nb x 5 Ni] contact-data gradients, solved as extra columns against the same factor
-DJ_DEV bool gradients(Ctx& c, double* __restrict__ Fz, double* __restrict__ Fu, double* __restrict__ Fc) {
+// u (nullable): this environment's inputs; null leaves the inputs' configuration derivative out (SURVEY.md Q17)
+DJ_DEV bool gradients(Ctx& c, const double* __restrict__ u, double* __restrict__ Fz, double* __restrict__ Fu, double* __restrict__ Fc) {
   const Plan& P = *c.P;
   double* A = c.A;
   const WarpRole& role = c.roles[c.warp];
@@ -693,7 +718,7 @@ DJ_DEV bool gradients(Ctx& c, double* __restrict__ Fz, double* __restrict__ Fu, 
     if (idx < 0) continue;
     if (role.type[p] == ROLE_BODY) grad_body(c, idx);
     else if (role.type[p] == ROLE_CONTACT) grad_contact(c, idx);
-    else grad_joint(c, idx);
+    else grad_joint(c, idx, u);
   }
   // per-column forward scratch must start from zero
   for (int j = c.tid; j < P.Ne; j += c.nthreads)

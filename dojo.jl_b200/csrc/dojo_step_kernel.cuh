@@ -312,7 +312,8 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
       }
       status = a.status ? a.status[e] : 0;
       const size_t ng = 12 * (size_t)P.Nb;
-      if (!gradients(c, a.Fz + (size_t)e * ng * ng, a.Fu + (size_t)e * ng * P.nu, a.Fc ? a.Fc + (size_t)e * ng * 5 * P.Ni : nullptr) && status == 0) status = 3;
+      const double* ug = (a.flags & DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN) ? nullptr : u;
+      if (!gradients(c, ug, a.Fz + (size_t)e * ng * ng, a.Fu + (size_t)e * ng * P.nu, a.Fc ? a.Fc + (size_t)e * ng * 5 * P.Ni : nullptr) && status == 0) status = 3;
     }
     if (a.sol) {  // reference ordering: joints [tra eq | s | gamma | rot eq] | bodies | contacts (device layout keeps eq rows first)
       double* so = a.sol + (size_t)e * P.nres;

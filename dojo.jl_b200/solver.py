@@ -17,6 +17,7 @@ LIB_PATH = os.path.join(_HERE, "libdojo_b200.so")
 
 DOJO_FLAG_Q1_LITERAL_RETURN = 1
 DOJO_FLAG_Q2_LITERAL_GRADIENTS = 2  # get_maximal_gradients! literally: data Jacobian after update_state! (include/dojo_b200.h)
+DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN = 4  # data Jacobian without d(input impulse)/d(configuration), as gradients/data.jl (include/dojo_b200.h)
 STATUS = {0: "success", 1: "failed", 2: "excessive_angular_velocity", 3: "nonfinite"}
 
 EXPORTS = ["dojo_default_options", "dojo_create", "dojo_destroy", "dojo_last_error", "dojo_num_state", "dojo_num_input",

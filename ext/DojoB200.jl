@@ -117,14 +117,17 @@ function Dojo.step!(mech::Mechanism, Z::Matrix{Float64}, U::Matrix{Float64}; opt
 end
 
 "batched get_maximal_gradients!.  literal_q2 = true reproduces what the single-environment get_maximal_gradients! literally returns (data
- Jacobian built after update_state!, gradients/state.jl:69-76; DOJO_FLAG_Q2_LITERAL_GRADIENTS); the default is the consistent IFT gradient."
-function Dojo.get_maximal_gradients!(mech::Mechanism, Z::Matrix{Float64}, U::Matrix{Float64}; opts = SolverOptions{Float64}(), literal_q2 = false)
+ Jacobian built after update_state!, gradients/state.jl:69-76; DOJO_FLAG_Q2_LITERAL_GRADIENTS); the default is the consistent IFT gradient.
+ literal_q17 = true leaves d(input impulse)/d(configuration) out of the data Jacobian as gradients/data.jl does
+ (DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN = 4); the reference's get_maximal_gradients! literally is literal_q2 = literal_q17 = true (flags 2 | 4)."
+function Dojo.get_maximal_gradients!(mech::Mechanism, Z::Matrix{Float64}, U::Matrix{Float64}; opts = SolverOptions{Float64}(), literal_q2 = false,
+                                     literal_q17 = false)
     h = handle(mech); B = size(Z, 2)
     Zn = similar(Z); Fz = zeros(h.ng, h.ng, B); Fu = zeros(h.ng, h.nu, B)
     status = zeros(Int32, B); iters = zeros(Int32, B)
     rc = ccall((:dojo_step_grad, LIB), Cint,
                (Ptr{Cvoid}, Ref{COptions}, Cint, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}, Ptr{Int32}, UInt32),
-               h.ptr, COptions(opts), B, Z, U, C_NULL, Zn, Fz, Fu, status, iters, literal_q2 ? 2 : 0)
+               h.ptr, COptions(opts), B, Z, U, C_NULL, Zn, Fz, Fu, status, iters, (literal_q2 ? 2 : 0) | (literal_q17 ? 4 : 0))
     rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
     return Fz, Fu
 end

@@ -88,6 +88,11 @@ extern "C" {
  * iterate (src/solver/mehrotra.jl:66-69).  Without the flag the consistent implicit-function-theorem gradient is
  * returned (data Jacobian and KKT matrix at the same state), which is what test/data.jl and the documentation pin. */
 #define DOJO_FLAG_Q2_LITERAL_GRADIENTS 2u
+/* dojo_step_grad*: leave d(input impulse)/d(x2, q2) out of the data Jacobian, as the
+ * reference's src/gradients/data.jl does (SURVEY Q17: input_jacobian_configuration of src/joints/{translational,rotational}/
+ * input.jl is defined but never called).  Without the flag, Fz is the derivative of the step the library computes, also at
+ * nonzero inputs when an actuated joint has a free parent.  Orthogonal to Q2: get_maximal_gradients! literally is Q2 | Q17. */
+#define DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN 4u
 
 /* Body: src/bodies/constructor.jl:13-27 (mass, inertia) */
 typedef struct {

@@ -59,6 +59,7 @@ struct JointS {  // joints/constraints.jl:17-86
   int eoff[2] = {0, 0};
   bool spring = false, damper = false;
   std::vector<double> imp[2];
+  V3 applied[2];  // the scaled input of the last set_input: translational force, rotational torque (joint frame)
 };
 
 struct ContactS {  // contacts/constructor.jl:14-43 + {nonlinear.jl:12-48, linear.jl:10-47, impact.jl:8-39} + sphere_halfspace.jl:11-24
@@ -560,6 +561,7 @@ struct Oracle {
   std::vector<std::pair<int, int>> pattern;          // structurally non-zero (node, node) blocks incl. fill
   bool tree_ok = true;
   int solver_mode = 0;  // 0 block LDU (reference-like), 1 dense partial-pivot LU
+  uint32_t grad_flags = 0;  // DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN: the data Jacobian omits d(input impulse)/d(configuration)
   std::vector<double> F;  // factor storage (copy of A)
 
   // diagnostics of the last mehrotra call
@@ -1007,6 +1009,7 @@ struct Oracle {
       Cfg a = cfg_current(j.parent, 1), b = cfg_current(j.child, 1);
       {  // translational
         V3 input = j.el[0].input * input_scaling;
+        j.applied[0] = input;
         Mat<6, 3> Ta = impulse_transform(true, j, 0, a.x, a.q, b.x, b.q);
         Mat<6, 3> Tb = impulse_transform(false, j, 0, a.x, a.q, b.x, b.q);
         V6 ia = Ta * input, ib = Tb * input;
@@ -1016,6 +1019,7 @@ struct Oracle {
       }
       {  // rotational
         V3 tau = j.el[1].input * input_scaling;
+        j.applied[1] = tau;
         if (j.parent >= 0) bodies[j.parent].Jt2 += vector_rotate(-tau, j.qoff);
         bodies[j.child].Jt2 += vector_rotate(tau, inv(b.q) * a.q * j.qoff);
         j.el[1].input = V3();
@@ -1842,6 +1846,10 @@ struct Oracle {
             ab += damper_jacobian_configuration(parent, !parent, j, k, a, b);
           }
         }
+        if (!(grad_flags & DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN)) {
+          aa += input_jacobian_configuration(parent, parent, j, a, b);
+          ab += input_jacobian_configuration(parent, !parent, j, a, b);
+        }
         int ob = body_off[bi];
         add(ob, colx(bi), 6, 3, [&](int r, int c) { return aa(r, c); });
         add(ob, colq(bi), 6, 3, [&](int r, int c) { return aa(r, 3 + c); });
@@ -1866,6 +1874,21 @@ struct Oracle {
       add(c.sol_off + c.nh, colx(c.body), c.nh, 3, [&](int r, int cc) { return Zc(r, cc); });
       add(c.sol_off + c.nh, colq(c.body), c.nh, 3, [&](int r, int cc) { return Zc(r, 3 + cc); });
     }
+  }
+  // d(input impulse)/d(x2, φ2) of the impulse set_input applies (SURVEY Q17; the reference's unused input_jacobian_configuration,
+  // translational/input.jl:45, rotational/input.jl:41): the translational input acts like a joint impulse with only half of its
+  // torque (Q16); the rotational input is a constant joint-frame torque, so only the child's R(qb⁻¹ qa qoff) depends on the poses.
+  M66 input_jacobian_configuration(bool parent, bool jac_parent, const JointS& j, const Cfg& a, const Cfg& b) const {
+    M66 out = impulse_transform_jacobian(parent, jac_parent, j, 0, a.x, a.q, b.x, b.q, j.applied[0]);
+    for (int r = 3; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) out(r, c) *= 0.5;
+    if (!parent) {
+      M33 Q = jac_parent ? M33(rotation_matrix(inv(b.q)) * drotation_matrix_dq(a.q, vector_rotate(j.applied[1], j.qoff)) * LVtmat(a.q))
+                         : M33(drotation_matrix_inv_dq(b.q, vector_rotate(j.applied[1], a.q * j.qoff)) * LVtmat(b.q));
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) out(3 + r, 3 + c) += Q(r, c);
+    }
+    return out;
   }
   // translational/springs.jl:44-60, rotational/springs.jl:44-84 (attjac = true): 6 x 6
   M66 spring_jacobian_configuration(bool parent, bool jac_parent, const JointS& j, int k, const V3& xa, const Quat& qa, const V3& xb,
@@ -2210,6 +2233,7 @@ void oracle_step_grad_batch_threads(const DojoMechanismDesc* d, const DojoSolver
         int it = 0;
         int st = o.step(*opts, Z + (size_t)e * nz, U + (size_t)e * o.nu, nullptr, Zn + (size_t)e * nz, nullptr, &it, flags);
         if (flags & DOJO_FLAG_Q2_LITERAL_GRADIENTS) o.update_state();
+        o.grad_flags = flags;
         double* pz = Fz ? Fz + (size_t)e * ns * ns : fz.data();
         double* pu = Fu ? Fu + (size_t)e * ns * o.nu : fu.data();
         if (!o.maximal_gradients(pz, pu, use_factor != 0) && st == 0) st = DOJO_STATUS_NONFINITE;
@@ -2229,6 +2253,7 @@ int oracle_step_grad(void* h, const DojoSolverOptions* opts, const double* z, co
   // DOJO_FLAG_Q2_LITERAL_GRADIENTS: get_maximal_gradients! = step! (incl. update_state!) THEN get_maximal_gradients (gradients/state.jl:69-76);
   // the KKT matrix `A` keeps the entries of the last set_entries! (the unshifted final iterate, solver/mehrotra.jl:66-69)
   if (flags & DOJO_FLAG_Q2_LITERAL_GRADIENTS) o->update_state();
+  o->grad_flags = flags;
   if (!o->maximal_gradients(Fz, Fu, use_factor != 0)) return DOJO_STATUS_NONFINITE;
   return st;
 }
@@ -2273,8 +2298,9 @@ int oracle_linear_solve(void* h, int mode, double* x, int m) {
   o->solver_mode = old;
   return ok ? 0 : -1;
 }
-void oracle_data_jacobian(void* h, double* out) {  // nres x (12Nb + nu) row-major
+void oracle_data_jacobian(void* h, double* out, uint32_t flags) {  // nres x (12Nb + nu) row-major
   Oracle* o = static_cast<Oracle*>(h);
+  o->grad_flags = flags;
   std::vector<double> D; o->data_jacobian(D);
   std::memcpy(out, D.data(), sizeof(double) * D.size());
 }

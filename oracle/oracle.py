@@ -61,7 +61,7 @@ def lib():
         L.oracle_violations.argtypes = [vp, dp, dp]
         L.oracle_linear_solve.argtypes = [vp, C.c_int, dp, C.c_int]
         L.oracle_linear_solve.restype = C.c_int
-        L.oracle_data_jacobian.argtypes = [vp, dp]
+        L.oracle_data_jacobian.argtypes = [vp, dp, C.c_uint32]
         L.oracle_trace.argtypes = [vp, dp, C.c_int]
         L.oracle_trace.restype = C.c_int
         L.oracle_momentum.argtypes = [vp, dp]
@@ -242,9 +242,11 @@ class Oracle:
             raise np.linalg.LinAlgError("singular block")
         return x
 
-    def data_jacobian(self):
+    def data_jacobian(self, flags=0):
+        """d(rhs)/d[state, input] at the current state, input and solution; flags: DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN omits the
+        inputs' configuration derivative as the reference's gradients/data.jl does."""
         out = np.empty((self.nres, 12 * self.mech.Nb + self.nu))
-        self.L.oracle_data_jacobian(self.h, _d(out))
+        self.L.oracle_data_jacobian(self.h, _d(out), int(flags))
         return out
 
     def trace(self):

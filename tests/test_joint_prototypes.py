@@ -45,12 +45,15 @@ def _moving_state(m, steps=8):
     return z, u
 
 
-@pytest.mark.parametrize("joint_type", list(PROTOTYPES))
-def test_oracle_blocks_match_finite_differences(joint_type):
+@pytest.mark.parametrize("joint_type,inputs", [pytest.param(t, "zero", id=t) for t in PROTOTYPES] +
+                         [pytest.param(t, "nonzero", id=f"{t}-inputs") for t in PROTOTYPES])
+def test_oracle_blocks_match_finite_differences(joint_type, inputs):
+    """KKT matrix and data Jacobian of the oracle == central differences of its residual.  With nonzero inputs the state columns
+    carry d(input impulse)/d(x2, q2) of every translational / rotational input, applied between a floating parent and its child."""
     m = snake(joint_type)
-    z, _ = _moving_state(m)
+    z, u = _moving_state(m)
     o = Oracle(m, capi.solver_options(rtol=1e-9, btol=1e-9))
-    u0 = np.zeros(m.nu)
+    u0 = np.zeros(m.nu) if inputs == "zero" else u
     _, _, _, sol = o.step(z, u0, return_sol=True)
     o.set_state(z, u0)
     o.set_solution(sol, 0.0)

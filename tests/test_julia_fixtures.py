@@ -97,14 +97,14 @@ def compare_with_oracle(mech, d, tol_z=1e-8, tol_mat=1e-9, tol_grad=1e-6, max_ca
         A, _ = o.assemble(0.0)
         Ar = np.asarray(case["solmat"], dtype=float).reshape(nres, nres, order="F")[np.ix_(ridx, ridx)]  # Julia vec() is column-major
         worst["solmat"] = max(worst["solmat"], np.abs(A - Ar).max() / np.abs(Ar).max())
-        _, Fz, Fu, _, _ = o.step_grad(z, u)
+        _, Fz, Fu, _, _ = o.step_grad(z, u, flags=4)  # the reference omits d(input impulse)/d(configuration) (SURVEY Q17)
         Fzr = np.asarray(case["Fz"], dtype=float).reshape(ns, ns, order="F")[np.ix_(sidx, sidx)]
         Fur = np.asarray(case["Fu"], dtype=float).reshape(ns, nu, order="F")[np.ix_(sidx, uidx)] if nu else np.zeros((ns, 0))
         worst["Fz"] = max(worst["Fz"], np.linalg.norm(Fz - Fzr) / max(1e-300, np.linalg.norm(Fzr)))
         if nu:
             worst["Fu"] = max(worst["Fu"], np.linalg.norm(Fu - Fur) / max(1e-300, np.linalg.norm(Fur)))
-        if "Fz_literal" in case:  # get_maximal_gradients! literally (DOJO_FLAG_Q2_LITERAL_GRADIENTS)
-            _, Fzl, Ful, _, _ = o.step_grad(z, u, flags=2)
+        if "Fz_literal" in case:  # get_maximal_gradients! literally (DOJO_FLAG_Q2_LITERAL_GRADIENTS | DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN)
+            _, Fzl, Ful, _, _ = o.step_grad(z, u, flags=2 | 4)
             Fzlr = np.asarray(case["Fz_literal"], dtype=float).reshape(ns, ns, order="F")[np.ix_(sidx, sidx)]
             worst["Fz"] = max(worst["Fz"], np.linalg.norm(Fzl - Fzlr) / max(1e-300, np.linalg.norm(Fzlr)))
     assert worst["z_next"] <= tol_z and worst["sol"] <= 1e-6 and worst["solmat"] <= tol_mat and worst["Fz"] <= tol_grad and worst["Fu"] <= tol_grad, worst
@@ -136,13 +136,13 @@ def synthetic_fixture(mech, ncases, seed):
             k += j.input_dimension
         zn, st, it, sol = o.step(z, u, return_sol=True)
         A, _ = o.assemble(0.0)
-        _, Fz, Fu, _, _ = o.step_grad(z, u)
+        _, Fz, Fu, _, _ = o.step_grad(z, u, flags=4)
         zq = o.step(z, u, flags=1)[0]
         cases.append({"z": zshuf(z).tolist(), "u": u[uidx].tolist(), "status": "success" if st == 0 else "failed", "sol": sol[ridx].tolist(),
                       "z_next": zshuf(zn).tolist(), "z_next_q1": zshuf(zq).tolist(),
                       "solmat": A[np.ix_(ridx, ridx)].reshape(-1, order="F").tolist(),
                       "Fz": Fz[np.ix_(sidx, sidx)].reshape(-1, order="F").tolist(), "Fu": Fu[np.ix_(sidx, uidx)].reshape(-1, order="F").tolist(),
-                      "Fz_literal": o.step_grad(z, u, flags=2)[1][np.ix_(sidx, sidx)].reshape(-1, order="F").tolist()})
+                      "Fz_literal": o.step_grad(z, u, flags=2 | 4)[1][np.ix_(sidx, sidx)].reshape(-1, order="F").tolist()})
         z = zn
     return {"body_names": [mech.bodies[b].name for b in bp], "joint_names": [mech.joints[j].name for j in jp],
             "contact_names": [mech.contacts[c].name for c in cp], "timestep": mech.timestep, "cases": cases}

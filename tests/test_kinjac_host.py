@@ -115,24 +115,43 @@ def test_minimal_gradients_device_code_on_host_matches_oracle(name):
 
 
 def test_minimal_gradients_match_finite_differences_of_the_minimal_step():
-    """get_minimal_gradients! is the derivative of step_minimal_coordinates! (pendulum with a tight solve: no contacts,
-    so the step is smooth)."""
-    mech = dj.get_mechanism("pendulum")
+    """get_minimal_gradients! is the derivative of step_minimal_coordinates! (a tight solve and no active contact, so the step is
+    smooth: the pendulum, and ant / quadruped / raiberthopper lifted 3 m with random inputs on every actuated joint, where the inputs'
+    configuration derivative (SURVEY Q17) belongs to Fz.  In minimal coordinates it shows for raiberthopper's prismatic leg, whose
+    input torque has a lever arm that moves along the joint; a revolute joint's input torque lies on its own axis.)"""
+    for name in ("pendulum", "ant", "quadruped", "raiberthopper"):
+        _minimal_gradients_match_finite_differences(name)
+
+
+def _minimal_gradients_match_finite_differences(name):
+    from conftest import random_inputs
+    mech = dj.get_mechanism(name)
     opts = capi.solver_options(rtol=1e-11, btol=1e-11)
     o = Oracle(mech, opts)
-    x = np.array([0.7, -0.4])
-    u = np.array([0.3])
+    if name == "pendulum":
+        x = np.array([0.7, -0.4])
+        u = np.array([0.3])
+    else:
+        rng = np.random.default_rng(4)
+        x = _random_minimal(mech, rng, 0.2, 0.5)
+        x[2] += 3.0  # floating base height
+        u = random_inputs(mech, 1, rng)[0]
 
     def f(x_, u_):
-        zn, st, _ = o.step(o.minimal_to_maximal(x_), u_)
+        zn, st, it = o.step(o.minimal_to_maximal(x_), u_)
         assert st == 0
-        return o.maximal_to_minimal(zn)
+        return o.maximal_to_minimal(zn), it
 
-    xn, Gx, Gu, st, _ = o.minimal_gradients(x, u)
-    assert st == 0 and np.abs(xn - f(x, u)).max() < 1e-12
-    eps = 1e-6
-    for i in range(2):
-        d = np.zeros(2)
+    xn, Gx, Gu, st, it0 = o.minimal_gradients(x, u)
+    assert st == 0 and np.abs(xn - f(x, u)[0]).max() < 1e-12
+    eps, n, checked = 1e-6, 2 * mech.nu, 0
+    for i in range(n + mech.nu):
+        d = np.zeros(n + mech.nu)
         d[i] = eps
-        assert np.abs((f(x + d, u) - f(x - d, u)) / (2 * eps) - Gx[:, i]).max() < 1e-6
-    assert np.abs((f(x, u + eps) - f(x, u - eps)) / (2 * eps) - Gu[:, 0]).max() < 1e-6
+        (fp, ip), (fm, im) = f(x + d[:n], u + d[n:]), f(x - d[:n], u - d[n:])
+        if ip != it0 or im != it0:
+            continue  # a different Newton-iteration count changes the (tolerance-level) solver error: FD noise / eps
+        G = Gx[:, i] if i < n else Gu[:, i - n]
+        assert np.abs((fp - fm) / (2 * eps) - G).max() < 1e-6 * max(1.0, np.abs(G).max()), (name, i, np.abs((fp - fm) / (2 * eps) - G).max())
+        checked += 1
+    assert checked >= (n + mech.nu) // 2, name

@@ -65,9 +65,15 @@ def _perturb_state(z, i, eps):
     return z2
 
 
-@pytest.mark.parametrize("name,steps,spring,damper", [("pendulum", 5, 1.0, 0.2), ("ant", 30, None, None), ("quadruped", 40, 0.3, 0.1), ("atlas", 3, None, None)])
-def test_data_jacobian_matches_finite_difference(name, steps, spring, damper):
-    """test/data.jl evaluates the finite differences with zero inputs (joint.input is cleared by input_impulse!)."""
+DATA_CASES = [("pendulum", 5, 1.0, 0.2), ("ant", 30, None, None), ("quadruped", 40, 0.3, 0.1), ("atlas", 3, None, None), ("cartpole", 5, None, None),
+              ("raiberthopper", 5, None, None)]
+
+
+@pytest.mark.parametrize("name,steps,spring,damper,u_value", [pytest.param(*c, 0.0, id="-".join(map(str, c))) for c in DATA_CASES] +
+                         [pytest.param(*c, 0.5, id="-".join(map(str, c)) + "-u0.5") for c in DATA_CASES])
+def test_data_jacobian_matches_finite_difference(name, steps, spring, damper, u_value):
+    """test/data.jl evaluates the finite differences with zero inputs (joint.input is cleared by input_impulse!).  With
+    u = 0.5 on every input the state columns also carry d(input impulse)/d(x2, q2), which the reference omits (SURVEY Q17)."""
     mech = dj.get_mechanism(name)
     if spring is not None:
         for j in mech.joints:
@@ -79,7 +85,7 @@ def test_data_jacobian_matches_finite_difference(name, steps, spring, damper):
     if mech.joints[0].nimpulses == 0:
         u0[:6] = 0
     z = _advance(o, mech, mech.z0.copy(), u0, steps)
-    u = np.zeros(mech.nu)
+    u = u_value * np.ones(mech.nu)
     _, _, _, sol = o.step(z, u, return_sol=True)
     mu = o.trace()[-1, 3]
     mu = 0.0 if mu != mu else mu
@@ -189,14 +195,29 @@ def _reduce(zz, zref, Nb):
     return np.concatenate(out)
 
 
-@pytest.mark.parametrize("name,steps", [("pendulum", 10), ("ant", 3)])
-def test_ift_gradients_match_finite_difference(name, steps):
-    """get_maximal_gradients (consistent IFT at the solution, SURVEY Q2) vs central differences of the step itself.
-    u = 0: the reference's data Jacobian omits d(input impulse)/d(q2) (it is never exercised by its tests)."""
+def _lift(z, height):
+    z = z.copy().reshape(-1, 13)
+    z[:, 2] += height
+    return z.reshape(-1)
+
+
+# (mechanism, roll-in steps from z0 with u = 0, lift of every body before the roll-in, input scale, solver tolerance)
+IFT_CASES = [pytest.param("pendulum", 10, 0.0, 0.0, 1e-10, id="pendulum-10"), pytest.param("ant", 3, 0.0, 0.0, 1e-10, id="ant-3"),
+             pytest.param("pendulum", 10, 0.0, 1.0, 1e-10, id="pendulum-10-u1"), pytest.param("ant", 3, 0.0, 1.0, 1e-10, id="ant-3-u1"),
+             pytest.param("ant", 2, 3.0, 1.0, 1e-10, id="ant-airborne-u1"), pytest.param("quadruped", 2, 3.0, 1.0, 1e-10, id="quadruped-airborne-u1"),
+             pytest.param("raiberthopper", 2, 3.0, 1.0, 1e-10, id="raiberthopper-airborne-u1"),
+             pytest.param("quadruped", 40, 0.0, 0.3, 1e-11, id="quadruped-sticking-u0.3")]  # settled on sticking contacts
+
+
+@pytest.mark.parametrize("name,steps,lift,u_scale,tol", IFT_CASES)
+def test_ift_gradients_match_finite_difference(name, steps, lift, u_scale, tol):
+    """get_maximal_gradients (consistent IFT at the solution, SURVEY Q2) vs central differences of the step itself, at zero and at
+    random nonzero inputs U(-u_scale, u_scale) on the actuated joints: Fz includes d(input impulse)/d(x2, q2) (SURVEY Q17), which
+    the reference's data Jacobian omits.  The airborne cases lift the whole mechanism 3 m, so no contact is active."""
     mech = dj.get_mechanism(name)
-    o = Oracle(mech, capi.solver_options(rtol=1e-10, btol=1e-10))
-    u = np.zeros(mech.nu)
-    z = _advance(Oracle(mech), mech, mech.z0.copy(), u, steps)
+    o = Oracle(mech, capi.solver_options(rtol=tol, btol=tol))
+    u = random_inputs(mech, 1, np.random.default_rng(3), u_scale)[0]
+    z = _advance(Oracle(mech), mech, _lift(mech.z0, lift), np.zeros(mech.nu), steps)
     zn, Fz, Fu, st, it0 = o.step_grad(z, u)
     _, Fz2, Fu2, _, _ = o.step_grad(z, u, use_factor=True)
     assert st == 0

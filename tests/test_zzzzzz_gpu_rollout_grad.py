@@ -116,25 +116,43 @@ def test_minimal_equals_per_step_composition():
 
 
 def test_pendulum_chained_jacobian_matches_central_differences():
+    """the chained Gx of dojo_rollout_minimal_gradients == central differences of dojo_rollout.  Ant and raiberthopper start 3 m up
+    (no contact: a smooth step) with random inputs on every actuated joint, so Fz must carry d(input impulse)/d(configuration)
+    (SURVEY Q17); raiberthopper's prismatic leg is where that term shows in minimal coordinates (without it the relative error is
+    4e-2 there).  Their bound leaves room for the FD noise of rollouts whose Newton iterations stop at different iterates."""
+    for name in ("pendulum", "ant", "raiberthopper"):
+        _chained_jacobian_matches_central_differences(name)
+
+
+def _chained_jacobian_matches_central_differences(name):
     from dojo_jl_b200.solver import BatchedStepper
-    m = _mech("pendulum")
-    assert m.Ni == 0
-    st = BatchedStepper(m, 16)
-    opts = capi.solver_options(rtol=1e-10, btol=1e-10)
-    x0 = np.array([[0.7, -0.3]])
-    U = np.full((T, 1, m.nu), 0.2)
+    from test_oracle_properties import _random_minimal
+    m = _mech(name)
+    nm = 2 * m.nu
+    st = BatchedStepper(m, 2 * nm)
+    opts = capi.solver_options(rtol=1e-10, btol=1e-10) if name == "pendulum" else capi.solver_options(rtol=1e-11, btol=1e-11)
+    if name == "pendulum":
+        assert m.Ni == 0
+        x0 = np.array([[0.7, -0.3]])
+        U = np.full((T, 1, m.nu), 0.2)
+    else:
+        rng = np.random.default_rng(41)
+        x0 = _random_minimal(m, rng, 0.2, 0.5)[None]
+        x0[0, 2] += 3.0
+        U = random_inputs(m, T, rng, 1.0)[:, None]
     Xt, Gx, _, s, _ = st.rollout_minimal_gradients(x0, U, T, opts)
-    assert (s == 0).all()
-    J = np.eye(2)
+    assert (s == 0).all(), name
+    J = np.eye(nm)
     for t in range(T):
         J = Gx[t, 0] @ J
     eps = 1e-6
-    X = np.concatenate([x0 + eps * np.eye(2), x0 - eps * np.eye(2)])
-    Zf, s_any = st.rollout(st.minimal_to_maximal(X), np.repeat(U, 4, axis=1), T, opts)
+    X = np.concatenate([x0 + eps * np.eye(nm), x0 - eps * np.eye(nm)])
+    Zf, s_any = st.rollout(st.minimal_to_maximal(X), np.repeat(U, 2 * nm, axis=1), T, opts)
     assert (s_any == 0).all()
     Xf = st.maximal_to_minimal(Zf)
-    Jfd = ((Xf[:2] - Xf[2:]) / (2 * eps)).T
-    assert np.linalg.norm(J - Jfd) <= 1e-6 * np.linalg.norm(J), (J, Jfd)
+    Jfd = ((Xf[:nm] - Xf[nm:]) / (2 * eps)).T
+    assert np.linalg.norm(J - Jfd) <= (1e-6 if name == "pendulum" else 2e-5) * np.linalg.norm(J), (name, np.linalg.norm(J - Jfd) / np.linalg.norm(J))
+    st.close()
 
 
 def test_refusals():

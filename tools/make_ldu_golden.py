@@ -48,7 +48,8 @@ def run(key, name, over, seed):
         Zn, st, it, sol = emu.step(Z, U, slots=slots)
         p = f"{key}/{slots}/"
         out.update({p + "Zn": Zn, p + "status": st, p + "iters": it, p + "sol": sol})
-        g = emu.step_grad(Z, U, slots=slots, slots_grad=slots)
+        # DOJO_FLAG_Q17_LITERAL_INPUT_JACOBIAN: the stored digests predate the inputs' configuration derivative (SURVEY Q17)
+        g = emu.step_grad(Z, U, slots=slots, slots_grad=slots, flags=4)
         # the Jacobians by SHA-256 of their bytes (atlas: 372 x 372 per environment would make the file megabytes)
         out.update({p + "gZn": g[0], p + "Fz_sha256": digest(g[1]), p + "Fu_sha256": digest(g[2]), p + "gstatus": g[3], p + "giters": g[4]})
     return out
