@@ -255,6 +255,26 @@ def get_trajectory_gradients(mechanism: Mechanism, z0, U, opts=None, device: int
     return traj, Fz, Fu, status
 
 
+def get_trajectory_vjp(mechanism: Mechanism, z0, U, gZ, opts=None, device: int = 0):
+    """The vector-Jacobian product of simulate!(mechanism, T, ...) from z0 with the open-loop inputs U, without the Jacobians: the rollout
+    recorded on the device (dojo_rollout_tape), then one adjoint pass (dojo_rollout_vjp).  z0 [13Nb], U [T, nu], gZ [T+1, 12Nb] (the
+    cotangent of every state in the gradients' packing [x, v, phi, w] per body) -> (Z_traj [T+1, 13Nb], gZ0 [12Nb], gU [T, nu], status [T]
+    of every step).  gZ0 and gU are get_trajectory_gradients' Jacobians contracted with gZ:  lambda_T = gZ[T], gU[t] = Fu[t]' lambda_{t+1},
+    lambda_t = Fz[t]' lambda_{t+1} + gZ[t], gZ0 = lambda_0.  An environment whose backward pass meets a non-finite factorisation gets
+    status 3 at every step and NaN gradients.  Batched: z0 [B, 13Nb], U [T, B, nu], gZ [T+1, B, 12Nb]."""
+    single, Z0, U, T = _trajectory_inputs(z0, U)
+    gZ = np.asarray(gZ, dtype=float)
+    if single:
+        gZ = gZ.reshape(gZ.shape[0], 1, -1)
+    s = _stepper(mechanism, Z0.shape[0], device)
+    traj, tape, status, _ = s.rollout_tape(Z0, U, T, opts)
+    gZ0, gU, vst = s.rollout_vjp(traj, U, tape, gZ)
+    status = np.where(vst[None, :] != 0, vst[None, :], status)
+    if single:
+        return traj[:, 0], gZ0[0], gU[:, 0], status[:, 0]
+    return traj, gZ0, gU, status
+
+
 def get_minimal_trajectory_gradients(mechanism: Mechanism, x0, U, opts=None, device: int = 0):
     """get_trajectory_gradients in minimal coordinates (get_minimal_gradients! at every step): x0 [2nu], U [T, nu] -> (X_traj [T+1, 2nu],
     Gx [T, 2nu, 2nu], Gu [T, 2nu, nu], status [T]).  The rollout runs in maximal coordinates from minimal_to_maximal(x0); X_traj is its

@@ -1,0 +1,128 @@
+"""PyTorch autograd through a fused rollout: rollout(mechanism, Z0, U) is differentiable with respect to Z0 and U.
+
+    from dojo_jl_b200.autograd import rollout
+    Z_traj, status = rollout(mech, Z0, U)           # CUDA fp64: Z0 [B, 13Nb], U [T, B, nu] -> Z_traj [T+1, B, 13Nb], status [T, B]
+    loss = f(Z_traj); loss.backward()               # Z0.grad, U.grad
+
+The forward pass records the rollout on the device (dojo_rollout_tape: the trajectory and the final solver iterate of every step) on the
+current torch stream; the backward pass runs one adjoint pass over it (dojo_rollout_vjp), also on the current stream.  Nothing of size
+12Nb x 12Nb per step is formed.  The gradients are those of the implicit-function-theorem Jacobians dojo_rollout_grad returns.
+
+Quaternions.  A state holds each body's attitude as a unit quaternion q, and the library differentiates along attitude perturbations
+q (x) (1, d) (dz in [x, v, phi, w] per body, 12 entries).  With G(q) = d(q (x) (1, d)) / dd at d = 0 (4 x 3; the reference's LVᵀmat(q)):
+  * a cotangent qbar on a quaternion of Z_traj enters the adjoint pass as phibar = G(q)' qbar;
+  * the quaternion part of dL/dZ0 is returned as G(q0) phibar0, the gradient in the tangent space of the unit sphere at q0: its radial
+    component q0' (dL/dq0) is 0.  A loss that depends on |q0| (it should not: Z0's quaternions are unit) is not differentiated along it.
+to_attitude / from_attitude are these two maps; they take torch tensors or numpy arrays alike (the CPU tests use the numpy form).
+status [T, B] (not differentiable) is each step's solver status; an environment whose backward pass meets a non-finite factorisation gets
+NaN gradients.
+"""
+import numpy as np
+
+from .mechanism import Mechanism
+from .solver import BatchedStepper
+
+
+def _xp(a):
+    return np if isinstance(a, np.ndarray) else __import__("torch")
+
+
+def attitude_map(q):
+    """G(q) [..., 4, 3] = d(q (x) (1, d)) / dd for quaternions q [..., 4] = (s, x, y, z):  [-v'; s I + skew(v)]"""
+    xp = _xp(q)
+    s, x, y, z = q[..., 0], q[..., 1], q[..., 2], q[..., 3]
+    rows = [(-x, -y, -z), (s, -z, y), (z, s, -x), (-y, x, s)]
+    return xp.stack([xp.stack(r, -1) for r in rows], -2)
+
+
+def to_attitude(Z, gZ):
+    """cotangents in the state packing [x, v, q, w] per body (gZ [..., 13Nb], at the states Z [..., 13Nb]) -> the gradients' packing
+    [x, v, phi, w] (12Nb), phibar = G(q)' qbar"""
+    xp = _xp(gZ)
+    sh = gZ.shape[:-1]
+    g = gZ.reshape(sh + (-1, 13))
+    q = Z.reshape(sh + (-1, 13))[..., 6:10]
+    phi = xp.einsum("...ij,...i->...j", attitude_map(q), g[..., 6:10])
+    return xp.concatenate([g[..., :6], phi, g[..., 10:]], -1).reshape(sh + (-1,))
+
+
+def from_attitude(Z, g):
+    """the gradients' packing [x, v, phi, w] per body (g [..., 12Nb], at the states Z [..., 13Nb]) -> the state packing, qbar = G(q) phibar
+    (tangent to the unit sphere at q)"""
+    xp = _xp(g)
+    sh = g.shape[:-1]
+    g = g.reshape(sh + (-1, 12))
+    q = Z.reshape(sh + (-1, 13))[..., 6:10]
+    qb = xp.einsum("...ij,...j->...i", attitude_map(q), g[..., 6:9])
+    return xp.concatenate([g[..., :6], qb, g[..., 9:]], -1).reshape(sh + (-1,))
+
+
+_steppers = {}
+
+
+def _stepper(mech: Mechanism, B: int, device: int) -> BatchedStepper:
+    """one handle per (mechanism, device), replaced by a larger one when B outgrows it; a replaced handle stays alive while a recorded
+    rollout holds it for its backward pass"""
+    key = (id(mech), device)
+    s = _steppers.get(key)
+    if s is None or s.max_batch < B:
+        s = BatchedStepper(mech, max(B, 64), device)
+        _steppers[key] = s
+    return s
+
+
+def _function():
+    import torch
+
+    class Rollout(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, Z0, U, stepper, opts):
+            T, B = U.shape[0], U.shape[1]
+            dev = Z0.device
+            Z0c, Uc = Z0.detach().contiguous(), U.detach().contiguous()
+            Z_traj = torch.empty((T + 1, B, stepper.nz), dtype=torch.float64, device=dev)
+            tape = torch.empty((T, B, stepper.nres), dtype=torch.float64, device=dev)
+            status = torch.empty((T, B), dtype=torch.int32, device=dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            stepper.rollout_tape_device(Z0c.data_ptr(), Uc.data_ptr() if stepper.nu > 0 else None, Z_traj.data_ptr(), tape.data_ptr(), B, T, opts,
+                                        dstatus=status.data_ptr(), stream=stream)
+            ctx.save_for_backward(Z_traj, Uc, tape)
+            ctx.stepper = stepper
+            ctx.mark_non_differentiable(status)
+            return Z_traj, status
+
+        @staticmethod
+        def backward(ctx, gZ_traj, _gstatus):
+            Z_traj, U, tape = ctx.saved_tensors
+            s = ctx.stepper
+            T, B = tape.shape[0], tape.shape[1]
+            dev = Z_traj.device
+            if gZ_traj is None:
+                gZ_traj = torch.zeros_like(Z_traj)
+            g = to_attitude(Z_traj, gZ_traj.to(torch.float64)).contiguous()
+            gZ0 = torch.empty((B, s.ngrad), dtype=torch.float64, device=dev)
+            gU = torch.empty((T, B, s.nu), dtype=torch.float64, device=dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            s.rollout_vjp_device(Z_traj.data_ptr(), U.data_ptr() if s.nu > 0 else None, tape.data_ptr(), g.data_ptr(), gZ0.data_ptr(), B, T,
+                                 dgU=gU.data_ptr() if s.nu > 0 else None, stream=stream)
+            return from_attitude(Z_traj[0], gZ0), gU, None, None
+
+    return Rollout
+
+
+_Rollout = None
+
+
+def rollout(mechanism: Mechanism, Z0, U, opts=None):
+    """T open-loop steps of B environments, differentiable with respect to Z0 [B, 13Nb] and U [T, B, nu] (CUDA float64 tensors on one
+    device).  Returns (Z_traj [T+1, B, 13Nb] with Z_traj[0] = Z0, status [T, B] int32).  opts: capi.solver_options(...) or None."""
+    import torch
+    global _Rollout
+    if _Rollout is None:
+        _Rollout = _function()
+    if Z0.dtype != torch.float64 or U.dtype != torch.float64 or not Z0.is_cuda or U.device != Z0.device:
+        raise ValueError("rollout: Z0 and U must be float64 CUDA tensors on one device")
+    if Z0.dim() != 2 or U.dim() != 3 or U.shape[1] != Z0.shape[0] or Z0.shape[1] != mechanism.nz or U.shape[2] != mechanism.nu:
+        raise ValueError(f"rollout: Z0 [B, {mechanism.nz}] and U [T, B, {mechanism.nu}] expected, got {tuple(Z0.shape)} and {tuple(U.shape)}")
+    s = _stepper(mechanism, Z0.shape[0], Z0.device.index if Z0.device.index is not None else torch.cuda.current_device())
+    return _Rollout.apply(Z0, U, s, opts)

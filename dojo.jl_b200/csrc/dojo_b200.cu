@@ -59,6 +59,13 @@ static const void* step_fb_kernel_fn(bool any_contact, bool plan_smem) {
   if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<false, true, false, false, false, true>;
   return (const void*)dojo_step_kernel<false, false, false, false, false, true>;
 }
+// the adjoint kernel (dojo_rollout_vjp): the VJP variant of the gradient kernel of the same compilation and plan placement as k_grad
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_vjp_kernel();
+static const void* step_vjp_kernel_fn(bool any_contact, bool plan_smem) {
+  if (any_contact) return dojo_cm_step_vjp_kernel();
+  if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<true, true, false, false, false, false, true>;
+  return (const void*)dojo_step_kernel<true, false, false, false, false, false, true>;
+}
 
 // Order of the work queue.  A per-step launch ends when its slowest environment ends: an environment that stalls (ten line-search
 // trials per iteration up to max_iter, ~6 x the median time) and is dequeued late finishes alone.  Which environments stall is not
@@ -224,6 +231,9 @@ struct DojoHandle {
   double* d_lqr = nullptr;                         // grow-only staging of host-pointer dojo_lqr_backward calls
   size_t lqr_bytes = 0;
   bool lqr_ready = false;                          // dojo_lqr_backward_kernel has the device's shared-memory maximum
+  const void* k_vjp = nullptr;                     // adjoint kernel (VJP), set up by the first dojo_rollout_vjp call
+  double* d_vjp = nullptr;                         // grow-only staging of host-pointer dojo_rollout_tape / dojo_rollout_vjp calls
+  size_t vjp_bytes = 0;
   std::string err;
 };
 // Whether the forward kernel specialised for small mechanisms (dojo_step_kernel.cuh, SMALL) computes this handle's step exactly: the
@@ -1754,6 +1764,146 @@ extern "C" int dojo_rollout_minimal_gradients(DojoHandle* h, const DojoSolverOpt
     if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_riters, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   }
   leave_call(h, s);
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  return DOJO_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Reverse mode through a rollout: the recording rollout without the Jacobians (tape) and its adjoint pass (include/dojo_b200.h)
+// ------------------------------------------------------------------------------------------------------------
+// Shared by the host- and device-pointer entries of both calls: no launch before every check has passed
+static int tape_vjp_setup(DojoHandle* h, int B, int T, bool buffers, const char* who) {
+  if (!h) return DOJO_EINVAL;
+  if (B <= 0 || B > h->max_batch || T <= 0 || !buffers || (long long)B * (T + 1) > (long long)INT_MAX - 2) {
+    h->err = std::string(who) + ": bad arguments (B in 1..max_batch, T >= 1, B * (T + 1) < 2^31 - 2, the required buffers)";
+    return DOJO_EINVAL;
+  }
+  if (!h->grad_bytes) { h->err = std::string(who) + ": the gradient workspace does not fit in shared memory for this mechanism"; return DOJO_ENOMEM; }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  return DOJO_OK;
+}
+
+// the REC launch of dojo_rollout_grad without the gradient kernel and without publishing pairs: the caller's tape is its sol_raw
+static int launch_tape(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZ_traj, double* dtape,
+                       int32_t* dstatus, int32_t* diters, cudaStream_t s) {
+  int rc = ensure_rec_kernel(h);
+  if (rc == DOJO_OK && !dstatus) rc = ensure_rollout_grad_scratch(h, (size_t)B * T);  // the REC kernel always writes a status
+  if (rc != DOJO_OK) return rc;
+  enter_call(h, s);
+  if (dZ0 != dZ_traj) CUDA_TRY(h, cudaMemcpyAsync(dZ_traj, dZ0, (size_t)B * h->plan.nz * sizeof(double), cudaMemcpyDeviceToDevice, s));
+  rc = launch_rollout(h, opts, B, T, dZ_traj, dU, nullptr, dZ_traj + (size_t)B * h->plan.nz, dstatus ? dstatus : h->d_rstatus, s, diters, dtape);
+  if (rc == DOJO_OK) leave_call(h, s);
+  return rc;
+}
+
+static int launch_vjp(DojoHandle* h, int B, int T, const double* dZ_traj, const double* dU, const double* dtape, const double* dgZ, double* dgZ0,
+                      double* dgU, int32_t* dstatus, cudaStream_t s) {
+  if (!h->k_vjp) {
+    const void* k = step_vjp_kernel_fn(h->any_contact, h->plan_smem_mask_grad == 0xff);
+    CUDA_TRY(h, max_shared_memory(k, h->device));
+    h->k_vjp = k;
+  }
+  // the adjoint pass reads no solver option: it runs no Newton iteration
+  StepArgs a = step_args(h, nullptr, B, true);
+  a.Z = dZ_traj; a.U = dU; a.sol_raw = const_cast<double*>(dtape); a.status = dstatus; a.T = T;
+  a.vjp_gZ = dgZ; a.vjp_lam = dgZ0; a.vjp_gU = dgU;
+  enter_call(h, s);
+  CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
+  // plainly after whatever recorded the tape: step T - 1 is needed first
+  const int grid = std::min((B + h->slots_grad - 1) / h->slots_grad, h->sm_count * h->envs_per_sm_grad);
+  { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(h->k_vjp, dim3(grid), dim3(32 * h->nw * h->slots_grad), kargs, h->smem_grad, s)); }
+  CUDA_TRY(h, cudaGetLastError());
+  h->launches += 1;
+  leave_call(h, s);
+  return DOJO_OK;
+}
+
+extern "C" int dojo_rollout_tape_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZ_traj,
+                                       double* dtape, int32_t* dstatus, int32_t* diters, void* cuda_stream) {
+  int rc = tape_vjp_setup(h, B, T, dZ0 && dZ_traj && dtape, "dojo_rollout_tape_async");
+  if (rc != DOJO_OK) return rc;
+  return launch_tape(h, opts, B, T, dZ0, dU, dZ_traj, dtape, dstatus, diters, (cudaStream_t)cuda_stream);
+}
+
+// one grow-only buffer for the host-pointer entries, carved into the arrays of n[] (in doubles; absent arrays take no space)
+static int vjp_staging(DojoHandle* h, const size_t* n, int k, double** d) {
+  size_t total = 0;
+  for (int i = 0; i < k; ++i) total += n[i];
+  int rc = grow_buffer(h, (void**)&h->d_vjp, &h->vjp_bytes, std::max<size_t>(total, 1) * sizeof(double));
+  if (rc != DOJO_OK) return rc;
+  size_t off = 0;
+  for (int i = 0; i < k; ++i) { d[i] = n[i] ? h->d_vjp + off : nullptr; off += n[i]; }
+  return DOJO_OK;
+}
+
+extern "C" int dojo_rollout_tape(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const double* U, double* Z_traj,
+                                 double* tape, int32_t* status, int32_t* iters) {
+  int rc = tape_vjp_setup(h, B, T, Z0 && Z_traj && tape, "dojo_rollout_tape");
+  if (rc != DOJO_OK) return rc;
+  cudaStream_t s = h->stream;
+  if (is_device_ptr(Z0)) {
+    rc = launch_tape(h, opts, B, T, Z0, U, Z_traj, tape, status, iters, s);
+    if (rc != DOJO_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    return DOJO_OK;
+  }
+  const Plan& P = h->plan;
+  const size_t pairs = (size_t)B * T;
+  const bool has_u = U && P.nu > 0;
+  // [Z_traj | tape | U] and status / iterations in the rollout scratch of dojo_rollout_grad
+  const size_t n[3] = {(pairs + B) * P.nz, pairs * P.nres, has_u ? pairs * P.nu : 0};
+  double* d[3];
+  rc = vjp_staging(h, n, 3, d);
+  if (rc == DOJO_OK) rc = ensure_rollout_grad_scratch(h, pairs);
+  if (rc != DOJO_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(d[0], Z0, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
+  if (has_u) CUDA_TRY(h, cudaMemcpyAsync(d[2], U, n[2] * sizeof(double), cudaMemcpyHostToDevice, s));
+  rc = launch_tape(h, opts, B, T, d[0], d[2], d[0], d[1], h->d_rstatus, h->d_riters, s);
+  if (rc != DOJO_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(Z_traj, d[0], n[0] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(tape, d[1], n[1] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_rstatus, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_riters, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  return DOJO_OK;
+}
+
+extern "C" int dojo_rollout_vjp_async(DojoHandle* h, int B, int T, const double* dZ_traj, const double* dU, const double* dtape, const double* dgZ,
+                                      double* dgZ0, double* dgU, int32_t* dstatus, void* cuda_stream) {
+  int rc = tape_vjp_setup(h, B, T, dZ_traj && dtape && dgZ && dgZ0, "dojo_rollout_vjp_async");
+  if (rc != DOJO_OK) return rc;
+  return launch_vjp(h, B, T, dZ_traj, dU, dtape, dgZ, dgZ0, dgU, dstatus, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int dojo_rollout_vjp(DojoHandle* h, int B, int T, const double* Z_traj, const double* U, const double* tape, const double* gZ, double* gZ0,
+                                double* gU, int32_t* status) {
+  int rc = tape_vjp_setup(h, B, T, Z_traj && tape && gZ && gZ0, "dojo_rollout_vjp");
+  if (rc != DOJO_OK) return rc;
+  cudaStream_t s = h->stream;
+  if (is_device_ptr(Z_traj)) {
+    rc = launch_vjp(h, B, T, Z_traj, U, tape, gZ, gZ0, gU, status, s);
+    if (rc != DOJO_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(s));
+    return DOJO_OK;
+  }
+  const Plan& P = h->plan;
+  const size_t pairs = (size_t)B * T, ng = 12 * (size_t)P.Nb;
+  const bool has_u = U && P.nu > 0;
+  // [Z_traj | tape | U | gZ | gZ0 | gU | status]
+  const size_t n[7] = {(pairs + B) * P.nz, pairs * P.nres, has_u ? pairs * P.nu : 0, (pairs + B) * ng, B * ng, gU ? pairs * P.nu : 0,
+                       status ? ((size_t)B + 1) / 2 : 0};
+  double* d[7];
+  rc = vjp_staging(h, n, 7, d);
+  if (rc != DOJO_OK) return rc;
+  const double* src[4] = {Z_traj, tape, U, gZ};
+  for (int k = 0; k < 4; ++k)
+    if (n[k]) CUDA_TRY(h, cudaMemcpyAsync(d[k], src[k], n[k] * sizeof(double), cudaMemcpyHostToDevice, s));
+  int32_t* dst = (int32_t*)d[6];
+  rc = launch_vjp(h, B, T, d[0], d[2], d[1], d[3], d[4], d[5], dst, s);
+  if (rc != DOJO_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(gZ0, d[4], n[4] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (gU && n[5]) CUDA_TRY(h, cudaMemcpyAsync(gU, d[5], n[5] * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, dst, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(h, cudaStreamSynchronize(s));
   return DOJO_OK;
 }

@@ -32,3 +32,7 @@ extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_rec_ke
 extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_fb_kernel() {
   return (const void*)dj_cm::dojo_step_kernel<false, false, false, false, false, true>;
 }
+// the adjoint kernel of this compilation (dojo_rollout_vjp)
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_vjp_kernel() {
+  return (const void*)dj_cm::dojo_step_kernel<true, false, false, false, false, false, true>;
+}

@@ -743,4 +743,158 @@ DJ_DEV bool gradients(Ctx& c, const double* __restrict__ u, double* __restrict__
   return ok;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// (4) adjoint of the step (dojo_rollout_vjp): lambda' Fz and lambda' Fu for ONE cotangent lambda, without the Jacobians.
+// ---------------------------------------------------------------------------------------------------------
+// Column col of [Fz Fu] is  C K^-1 rhs_col + d_col  (grad_write_column): C maps the body rows of the condensed system to
+// (x3, v25, phi3, w25) -- dx = h dv, dphi = E dw -- and d_col is the direct term (e_k on the x2 columns, M e_k on the phi2 columns).
+// So  lambda' col = y' rhs_col + lambda' d_col  with  y = K^-T C' lambda:  one transposed solve instead of 12Nb + nu forward ones.
+//
+// The block LDU of the factorisation is K = L (D + U): L unit lower (L~_{nb,c} at ElimNb::L_off, applied by the forward sweep of
+// grad_solve_columns), D the pivots (their inverses at d_off), U the blocks M_{c,nb} at U_off (backward sweep).  K' y = g is solved as
+//   (D + U)' w = g   phases in FORWARD order:  w_c = Dinv_c' g_c, then g_nb -= M_{c,nb}' w_c   (the transposed backward sweep)
+//   L' y = w         phases in REVERSE order:  y_c = w_c - sum_nb L~_{nb,c}' y_nb              (the transposed forward sweep)
+// The first has the forward sweep's access pattern, so it reaches the same targets the same way: updates of a parent body go to the
+// per-joint scratch (ElimNb::gv_off, sub-range row0) that the parent folds in (ElimStep::gfold_off) when its own turn comes; the second
+// reads its neighbours where the backward sweep does.  One right-hand side: warp 0 runs it, one lane per step of a phase (y and the
+// scratch with stride 1: y in the residual region, which the gradient pass no longer needs once the KKT blocks are assembled).
+DJ_DEV void vjp_solve(Ctx& c, double* __restrict__ y) {
+  const Plan& P = *c.P;
+  double* A = c.A;
+  for (int ph = 0; ph < P.nphase; ++ph) {
+    const int s0 = c.sched[2 * (ph * P.nw)], s1 = c.sched[2 * (ph * P.nw + P.nw - 1)] + c.sched[2 * (ph * P.nw + P.nw - 1) + 1];
+    for (int s = s0 + c.lane; s < s1; s += 32) {
+      const ElimStep& st = c.steps[s];
+      double g[6], w[6];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) g[k] = (k < st.n) ? y[st.r_off + k] : 0.0;
+      for (int q = 0; q < st.fold_cnt; ++q) {
+        double* v = A + c.ilist[st.gfold_off + q];
+#pragma unroll
+        for (int k = 0; k < 6; ++k)
+          if (k < st.n) { g[k] += v[k]; v[k] = 0.0; }
+      }
+      const double* Dc = A + st.d_off;
+      bool nz = false;
+#pragma unroll
+      for (int r = 0; r < 6; ++r) {
+        w[r] = 0.0;
+        if (r < st.n) {
+          double acc = 0.0;
+#pragma unroll
+          for (int k = 0; k < 6; ++k)
+            if (k < st.n) acc += Dc[k * st.n + r] * g[k];
+          w[r] = acc;
+          y[st.r_off + r] = acc;
+          nz = nz || (acc != 0.0);
+        }
+      }
+      if (!nz) continue;
+      for (int j = 0; j < st.nnb; ++j) {
+        const ElimNb& nb = st.nb[j];
+        const double* U = A + nb.U_off;
+        double* tgt = nb.gv_off >= 0 ? A + nb.gv_off + nb.row0 : y + nb.r_off;
+        for (int kk = 0; kk < nb.n; ++kk) {
+          double acc = 0.0;
+          if (nb.U_row == 0) {  // M_{c,nb} holds all st.n rows of c
+#pragma unroll
+            for (int r = 0; r < 6; ++r)
+              if (r < st.n) acc += U[r * nb.n + kk] * w[r];
+          } else {  // angular coupling only: rows 3..5 of c, stored 3 x n_nb
+#pragma unroll
+            for (int r = 0; r < 3; ++r) acc += U[r * nb.n + kk] * w[3 + r];
+          }
+          tgt[kk] -= acc;
+        }
+      }
+    }
+    __syncwarp();
+  }
+  for (int ph = P.nphase - 1; ph >= 0; --ph) {
+    const int s0 = c.sched[2 * (ph * P.nw)], s1 = c.sched[2 * (ph * P.nw + P.nw - 1)] + c.sched[2 * (ph * P.nw + P.nw - 1) + 1];
+    for (int s = s0 + c.lane; s < s1; s += 32) {
+      const ElimStep& st = c.steps[s];
+      double t[6];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) t[k] = (k < st.n) ? y[st.r_off + k] : 0.0;
+      for (int j = 0; j < st.nnb; ++j) {
+        const ElimNb& nb = st.nb[j];
+        const double* L = A + nb.L_off;
+        const double* xj = y + nb.r_off;
+        for (int i = 0; i < nb.n; ++i) {
+          const double xv = xj[i];
+#pragma unroll
+          for (int k = 0; k < 6; ++k)
+            if (k < st.n) t[k] -= L[i * st.n + k] * xv;
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < 6; ++k)
+        if (k < st.n) y[st.r_off + k] = t[k];
+    }
+    __syncwarp();
+  }
+}
+
+// One step of the adjoint pass at the final iterate whose KKT blocks are assembled (unfactorised), as gradients() is called:
+// on entry lam [12 Nb] (global memory, this slot's only) holds lambda_{t+1}; on return lambda_t = Fz' lambda_{t+1} + gz, and gu [nu]
+// (nullable) = Fu' lambda_{t+1}.  u: the step's inputs (their configuration derivative is part of Fz, as in dojo_rollout_grad).
+// Every sum runs in a fixed order on one lane.  Returns false when the factorisation is not finite.
+DJ_DEV bool vjp_step(Ctx& c, const double* __restrict__ u, double* __restrict__ lam, const double* __restrict__ gz, double* __restrict__ gu) {
+  const Plan& P = *c.P;
+  double* A = c.A;
+  const WarpRole& role = c.roles[c.warp];
+  for (int p = 0; p < role.npass; ++p) {  // the data-Jacobian blocks of gradients()
+    const int idx = role_item(role, p, c.lane);
+    if (idx < 0) continue;
+    if (role.type[p] == ROLE_BODY) grad_body(c, idx);
+    else if (role.type[p] == ROLE_CONTACT) grad_contact(c, idx);
+    else grad_joint(c, idx, u);
+  }
+  for (int j = c.tid; j < P.Ne; j += c.nthreads)  // the transposed solve's scratch (stride 1) starts from zero
+    if (c.joints[j].gv_off >= 0)
+      for (int k = 0; k < 6; ++k) A[c.joints[j].gv_off + k] = 0.0;
+  double* y = A + P.rhs_off;
+  for (int r = c.tid; r < P.n_red; r += c.nthreads) y[r] = 0.0;
+  slot_sync(c);
+  const bool ok = factorize(c);
+  // right-hand side C' lambda on the body rows (zero on the joint rows): dv <- h lambda_x + lambda_v, dw <- E' lambda_phi + lambda_w.
+  // The thread of body b then replaces lambda's 12 entries of b by the direct terms (lambda_x on x2, M' lambda_phi on phi2, 0 elsewhere).
+  for (int b = c.tid; b < P.Nb; b += c.nthreads) {
+    const BodyDev& bd = c.bodies[b];
+    const double* rec = A + bd.gb_off;
+    double* l = lam + 12 * b;
+    const V3 lx = ld3(l), lv = ld3(l + 3), lp = ld3(l + 6), lw = ld3(l + 9);
+    st3(y + bd.r_off, P.h * lx + lv);
+    st3(y + bd.r_off + 3, tmul(ldm33(rec + 18), lp) + lw);
+    st3(l + 3, v3zero());
+    st3(l + 6, tmul(ldm33(rec + 9), lp));
+    st3(l + 9, v3zero());
+  }
+  __threadfence_block();
+  slot_sync(c);
+  if (c.warp == 0) vjp_solve(c, y);
+  slot_sync(c);
+  // lambda' col = y' rhs_col + (direct term), one lane per column, the columns built by grad_build_rhs in the chunks of gradients()
+  const int ng = 12 * P.Nb;
+  const int chw = P.ch / P.nw;
+  double* V = A + P.gvec_off + c.warp * P.n_red * chw;
+  const int part = c.lane / chw, l = c.lane - part * chw;
+  for (int c0 = c.warp * chw; c0 < P.ncol; c0 += P.ch) {
+    const int col = c0 + l;
+    if (part == 0 && col < P.ncol) grad_build_rhs(c, V, chw, col, l);
+    __syncwarp();
+    if (part == 0 && col < P.ncol) {
+      double s = 0.0;
+      for (int r = 0; r < P.n_red; ++r) s += y[r] * V[r * chw + l];
+      if (col < ng) lam[col] = (s + lam[col]) + gz[col];
+      else if (gu) gu[col - ng] = s;
+    }
+    __syncwarp();
+  }
+  __threadfence_block();
+  slot_sync(c);
+  return ok;
+}
+
 }  // namespace dj

@@ -67,7 +67,44 @@ struct StepArgs {
   double* fb_xi;  // [2nu x B] integral state, updated in place (required iff fb_Ki)
   double* fb_u;   // u_t, where prologue reads it: [nu x B x T] (fb_u_T = 1, the applied inputs) or [nu x B] scratch (fb_u_T = 0)
   int fb_u_T;
+  // adjoint of a recorded rollout (VJP kernels only, dojo_rollout_vjp): a.Z is the trajectory [nz x B x (T + 1)], a.U the inputs
+  // [nu x B x T] (nullable), a.sol_raw the tape [nres x B x T], a.status [B] (nullable).  Cotangents in the gradients' packing
+  // [x, v, phi, w] per body.  After fb_u_T, so that no other member moves.
+  const double* vjp_gZ;  // [12Nb x B x (T + 1)]
+  double* vjp_lam;       // [12Nb x B]: lambda_t of the step the owning slot is at; gZ0 = lambda_0 on return
+  double* vjp_gU;        // nullable [nu x B x T]
 };
+
+// adjoint pass of the VJP kernel for environment e (dojo_rollout_vjp): lambda_T = gZ[T]; for t = T-1 .. 0 the gradient pass's
+// prologue, tape and assembly at pair t * B + e, then vjp_step (dojo_grad.cuh): gU[t] = Fu_t' lambda_{t+1}, lambda_t = Fz_t' lambda_{t+1}
+// + gZ[t].  Returns the environment's status: 0, or 3 when a factorisation was not finite (its gZ0 and every gU[t] are then NaN).
+DJ_DEV int rollout_vjp(Ctx& c, const StepArgs& a, int e) {
+  const Plan& P = *c.P;
+  const int ng = 12 * P.Nb;
+  double* lam = a.vjp_lam + (size_t)e * ng;
+  const double* gT = a.vjp_gZ + ((size_t)a.T * a.B + e) * ng;
+  for (int k = c.tid; k < ng; k += c.nthreads) lam[k] = gT[k];
+  __threadfence_block();
+  slot_sync(c);
+  bool ok = true;
+  for (int t = a.T - 1; t >= 0 && ok; --t) {
+    const size_t p = (size_t)t * a.B + e;
+    const double* u = a.U ? a.U + p * P.nu : nullptr;
+    prologue(c, a.Z + p * P.nz, u, nullptr, true);
+    for (int k = c.tid; k < P.nres; k += c.nthreads) c.A[P.sol_off + k] = a.sol_raw[p * P.nres + k];
+    slot_sync(c);
+    double rv, bv;
+    c.mu = 0.0;
+    evaluate<true>(c, 0.0, P.rhs_off, rv, bv);
+    ok = vjp_step(c, u, lam, a.vjp_gZ + p * ng, a.vjp_gU ? a.vjp_gU + p * P.nu : nullptr);
+  }
+  if (ok) return 0;
+  const double qnan = nan("");
+  for (int k = c.tid; k < ng; k += c.nthreads) lam[k] = qnan;
+  if (a.vjp_gU)
+    for (int k = c.tid; k < a.T * P.nu; k += c.nthreads) a.vjp_gU[((size_t)(k / P.nu) * a.B + e) * P.nu + k % P.nu] = qnan;
+  return 3;
+}
 
 // feedback stage of the FB kernel for environment e before step t from state z (global memory); returns where u_t was written.
 // Lanes: one per joint for the map (max_to_min_joint reads only the joint's parent and child), one per entry of xi, one per input.
@@ -148,11 +185,15 @@ __device__ __forceinline__ unsigned long long k_t0g(unsigned long long* prof) { 
 // FB (forward, untraced, generic): the closed-loop rollout of dojo_rollout_feedback.  Before the prologue of step t the slot evaluates the
 // linear feedback law on the state the step starts from (feedback() above) and the step reads u_t from a.fb_u; a.U is not read.  The step
 // itself is dojo_rollout's.  A compile-time parameter, like REC.
-template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false, bool SMALL = false, bool REC = false, bool FB = false>
+// VJP (gradient): the adjoint pass of dojo_rollout_vjp.  A slot takes an environment from the work queue and walks its recorded steps
+// backwards (rollout_vjp() above), one transposed solve per step instead of the gradient kernel's column solves.  Same launch
+// configuration and arena as the gradient kernel; a compile-time parameter, so that the other instantiations are the same code.
+template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false, bool SMALL = false, bool REC = false, bool FB = false, bool VJP = false>
 __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(const StepArgs a) {
   static_assert(!SMALL || (!GRAD && PLAN_SMEM && !TRACE), "SMALL is a specialisation of the untraced forward kernel with the plan in shared memory");
   static_assert(!REC || (!GRAD && !TRACE && !SMALL), "REC is a variant of the generic untraced forward kernel");
   static_assert(!FB || (!GRAD && !TRACE && !SMALL && !REC), "FB is a variant of the generic untraced forward kernel");
+  static_assert(!VJP || (GRAD && !TRACE && !SMALL && !REC && !FB), "VJP is a variant of the gradient kernel");
   extern __shared__ double arena[];
   __shared__ __align__(8) int s_env[128];  // CTA-wide mailbox, layout: dojo_kernels.cuh (cta_align)
   // a CTA hosts a.slots environments at a time; slot k is served by threads [k * 32 nw, (k + 1) * 32 nw)
@@ -248,7 +289,9 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
 #endif
     const double* z = a.Z + (size_t)e * P.nz;
     int worst = 0, iters = 0, status = 0;
-    if (!GRAD) {
+    if (VJP) {
+      status = rollout_vjp(c, a, e);
+    } else if (!GRAD) {
       for (int t = 0; t < a.T; ++t) {
         const double* u = a.U ? a.U + ((size_t)t * a.B + e) * P.nu : nullptr;
         if (FB) u = feedback(c, a, z, e, t);

@@ -30,7 +30,8 @@ EXPORTS = ["dojo_default_options", "dojo_create", "dojo_destroy", "dojo_last_err
            "dojo_step_grad_contact_async", "dojo_step_record", "dojo_step_record_async", "dojo_simulate_record",
            "dojo_gather_create", "dojo_gather_export", "dojo_gather_connect", "dojo_gather_buffer", "dojo_gather_destroy", "dojo_step_gather_async",
            "dojo_step_grad_gather_async", "dojo_step_trace", "dojo_step_trace_async", "dojo_rollout_grad", "dojo_rollout_grad_async",
-           "dojo_rollout_minimal_gradients", "dojo_rollout_feedback", "dojo_rollout_feedback_async", "dojo_lqr_backward", "dojo_lqr_backward_async"]
+           "dojo_rollout_minimal_gradients", "dojo_rollout_feedback", "dojo_rollout_feedback_async", "dojo_lqr_backward", "dojo_lqr_backward_async",
+           "dojo_rollout_tape", "dojo_rollout_tape_async", "dojo_rollout_vjp", "dojo_rollout_vjp_async"]
 
 _lib = None
 
@@ -125,6 +126,14 @@ def load_library():
     L.dojo_rollout_grad_async.restype = C.c_int
     L.dojo_rollout_minimal_gradients.argtypes = [vp, op, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
     L.dojo_rollout_minimal_gradients.restype = C.c_int
+    L.dojo_rollout_tape.argtypes = [vp, op, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_tape.restype = C.c_int
+    L.dojo_rollout_tape_async.argtypes = [vp, op, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_tape_async.restype = C.c_int
+    L.dojo_rollout_vjp.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_vjp.restype = C.c_int
+    L.dojo_rollout_vjp_async.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_vjp_async.restype = C.c_int
     fp = C.POINTER(capi.DojoFeedback)
     L.dojo_rollout_feedback.argtypes = [vp, op, C.c_int, C.c_int, vp, fp, vp, vp, vp, vp, vp]
     L.dojo_rollout_feedback.restype = C.c_int
@@ -388,6 +397,42 @@ class BatchedStepper:
         rc = self.L.dojo_rollout_grad(self.h, C.byref(o), B, T, _p(Z0), _p(U), _p(traj), _p(Fz), _p(Fu), _p(status), _p(iters))
         self._check(rc, "dojo_rollout_grad")
         return traj, np.transpose(Fz, (0, 1, 3, 2)), np.transpose(Fu, (0, 1, 3, 2)), status, iters
+
+    def rollout_tape(self, Z0, U=None, T: int = 1, opts=None):
+        """The recording rollout of rollout_grad without the Jacobians (dojo_rollout_tape).  U [T, B, nu] or None.  Returns (Z_traj
+        [T+1, B, 13Nb], tape [T, B, nres], status [T, B], iters [T, B]); the tape is the final solver iterate of every step in the library's
+        internal ordering, read only by rollout_vjp."""
+        Z0 = np.ascontiguousarray(np.atleast_2d(Z0), dtype=np.float64)
+        B, T = Z0.shape[0], int(T)
+        assert Z0.shape[1] == self.nz
+        if U is not None:
+            U = np.ascontiguousarray(U, dtype=np.float64)
+            assert U.shape == (T, B, self.nu)
+        traj = np.empty((max(T, 0) + 1, B, self.nz))
+        tape = np.empty((max(T, 0), B, self.nres))
+        status, iters = np.zeros((max(T, 0), B), dtype=np.int32), np.zeros((max(T, 0), B), dtype=np.int32)
+        o = opts if opts is not None else capi.solver_options()
+        rc = self.L.dojo_rollout_tape(self.h, C.byref(o), B, T, _p(Z0), _p(U), _p(traj), _p(tape), _p(status), _p(iters))
+        self._check(rc, "dojo_rollout_tape")
+        return traj, tape, status, iters
+
+    def rollout_vjp(self, Z_traj, U, tape, gZ):
+        """Reverse-mode derivative of the rollout rollout_tape recorded (dojo_rollout_vjp): with lambda_T = gZ[T] and, for t = T-1 .. 0,
+        gU[t] = Fu_t' lambda_{t+1}, lambda_t = Fz_t' lambda_{t+1} + gZ[t] (Fz, Fu: rollout_grad's Jacobians), returns (gZ0 = lambda_0
+        [B, 12Nb], gU [T, B, nu], status [B]: 0, or 3 when a factorisation was not finite -- that environment's outputs are then NaN).
+        Cotangents are in the gradients' packing [x, v, phi, w] per body: gZ [T+1, B, 12Nb]."""
+        tape = np.ascontiguousarray(tape, dtype=np.float64)
+        T, B = tape.shape[0], tape.shape[1]
+        Z_traj = np.ascontiguousarray(Z_traj, dtype=np.float64)
+        gZ = np.ascontiguousarray(gZ, dtype=np.float64)
+        assert Z_traj.shape == (T + 1, B, self.nz) and tape.shape == (T, B, self.nres) and gZ.shape == (T + 1, B, self.ngrad)
+        if U is not None:
+            U = np.ascontiguousarray(U, dtype=np.float64)
+            assert U.shape == (T, B, self.nu)
+        gZ0, gU, status = np.empty((B, self.ngrad)), np.empty((T, B, self.nu)), np.zeros(B, dtype=np.int32)
+        rc = self.L.dojo_rollout_vjp(self.h, B, T, _p(Z_traj), _p(U), _p(tape), _p(gZ), _p(gZ0), _p(gU), _p(status))
+        self._check(rc, "dojo_rollout_vjp")
+        return gZ0, gU, status
 
     def rollout_minimal_gradients(self, X0, U=None, T: int = 1, opts=None):
         """The same in minimal coordinates (dojo_rollout_minimal_gradients): the rollout from minimal_to_maximal(X0) and
@@ -690,6 +735,22 @@ class BatchedStepper:
         rc = self.L.dojo_rollout_grad_async(self.h, C.byref(o), int(B), int(T), _p(dZ0), _p(dU), _p(dZ_traj), _p(dFz), _p(dFu), _p(dstatus),
                                             _p(diters), C.c_void_p(int(stream)))
         self._check(rc, "dojo_rollout_grad_async")
+
+    def rollout_tape_device(self, dZ0: int, dU: Optional[int], dZ_traj: int, dtape: int, B: int, T: int, opts=None, dstatus=None, diters=None,
+                            stream: int = 0):
+        """dojo_rollout_tape_async on device pointers: Z_traj [T+1, B, 13Nb], tape [T, B, nres], status / iters [T, B] (nullable); dZ0 may
+        be dZ_traj (slab 0 already holds Z0)."""
+        o = opts if opts is not None else capi.solver_options()
+        rc = self.L.dojo_rollout_tape_async(self.h, C.byref(o), int(B), int(T), _p(dZ0), _p(dU), _p(dZ_traj), _p(dtape), _p(dstatus), _p(diters),
+                                            C.c_void_p(int(stream)))
+        self._check(rc, "dojo_rollout_tape_async")
+
+    def rollout_vjp_device(self, dZ_traj: int, dU: Optional[int], dtape: int, dgZ: int, dgZ0: int, B: int, T: int, dgU=None, dstatus=None,
+                           stream: int = 0):
+        """dojo_rollout_vjp_async on device pointers: gZ [T+1, B, 12Nb] in, gZ0 [B, 12Nb] out, gU [T, B, nu] and status [B] (nullable)."""
+        rc = self.L.dojo_rollout_vjp_async(self.h, int(B), int(T), _p(dZ_traj), _p(dU), _p(dtape), _p(dgZ), _p(dgZ0), _p(dgU), _p(dstatus),
+                                           C.c_void_p(int(stream)))
+        self._check(rc, "dojo_rollout_vjp_async")
 
     def rollout_feedback_device(self, dZ0: int, dZf: int, B: int, T: int, dK: int, steps: int = 1, envs: int = 1, dK_i=None, dx_ref=None, du_ref=None,
                                 dxi=None, dtraj=None, dU_applied=None, dstatus=None, opts=None, stream: int = 0):

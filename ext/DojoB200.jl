@@ -293,6 +293,30 @@ function rollout_gradients(mech::Mechanism, Z0::Matrix{Float64}, U::Array{Float6
     rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
     return traj, Fz, Fu, status
 end
+"the recording rollout of rollout_gradients without the Jacobians: returns (Z_traj 13Nb x B x (T+1), tape nres x B x T -- the final solver
+ iterate of every step, read only by rollout_vjp -- status B x T)"
+function rollout_tape(mech::Mechanism, Z0::Matrix{Float64}, U::Array{Float64,3}; opts = SolverOptions{Float64}())
+    h = handle(mech); B = size(Z0, 2); T = size(U, 3)
+    nres = ccall((:dojo_num_residual, LIB), Cint, (Ptr{Cvoid},), h.ptr)
+    traj = zeros(h.nz, B, T + 1); tape = zeros(nres, B, T); status = zeros(Int32, B, T); iters = zeros(Int32, B, T)
+    rc = ccall((:dojo_rollout_tape, LIB), Cint,
+               (Ptr{Cvoid}, Ref{COptions}, Cint, Cint, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}, Ptr{Int32}),
+               h.ptr, COptions(opts), B, T, Z0, U, traj, tape, status, iters)
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return traj, tape, status
+end
+"reverse mode through the rollout rollout_tape recorded: gZ 12Nb x B x (T+1) (cotangents in the packing [x, v, phi, w] per body) ->
+ (gZ0 12Nb x B, gU nu x B x T, status B: 0, or 3 with NaN gradients when a factorisation was not finite), the contraction of
+ rollout_gradients' Fz / Fu:  lambda_T = gZ[T], gU[t] = Fu_t' lambda_{t+1}, lambda_t = Fz_t' lambda_{t+1} + gZ[t], gZ0 = lambda_0"
+function rollout_vjp(mech::Mechanism, Z_traj::Array{Float64,3}, U::Array{Float64,3}, tape::Array{Float64,3}, gZ::Array{Float64,3})
+    h = handle(mech); B = size(Z_traj, 2); T = size(tape, 3); ng = 12 * length(mech.bodies)
+    gZ0 = zeros(ng, B); gU = zeros(h.nu, B, T); status = zeros(Int32, B)
+    rc = ccall((:dojo_rollout_vjp, LIB), Cint,
+               (Ptr{Cvoid}, Cint, Cint, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}),
+               h.ptr, B, T, Z_traj, U, tape, gZ, gZ0, gU, status)
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return gZ0, gU, status
+end
 "the same in minimal coordinates (get_minimal_gradients! at every step): X_traj 2nu x B x (T+1), Gx 2nu x 2nu x B x T, Gu 2nu x nu x B x T"
 function rollout_minimal_gradients(mech::Mechanism, X0::Matrix{Float64}, U::Array{Float64,3}; opts = SolverOptions{Float64}())
     h = handle(mech); B = size(X0, 2); T = size(U, 3); nm = 2 * h.nu

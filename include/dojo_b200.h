@@ -23,6 +23,8 @@
  *                                   get_minimal_state and applies a time-varying linear law (examples/control)
  *   dojo_rollout_grad            <- simulate! + get_maximal_gradients! at every step
  *   dojo_rollout_minimal_gradients <- simulate! + get_minimal_gradients! at every step
+ *   dojo_rollout_tape + dojo_rollout_vjp <- simulate! + get_maximal_gradients! at every step, contracted with a loss gradient
+ *                                   (the vector-Jacobian product, without the Jacobians)
  *   dojo_lqr_backward            <- the backward pass of IterativeLQR.jl's solve! (iLQR / TVLQR gains
  *                                   from the minimal-coordinate Jacobians and a quadratic cost;
  *                                   docs/src/examples/trajectory_optimization.md)
@@ -418,6 +420,32 @@ int dojo_rollout_grad_async(DojoHandle* h, const DojoSolverOptions* opts, int B,
  * maximal states never leave the device).  Host or device pointers (all of the same kind). */
 int dojo_rollout_minimal_gradients(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* X0, const double* U,
                                    double* X_traj, double* Gx, double* Gu, int32_t* status, int32_t* iters);
+
+/* Reverse mode through a rollout: a loss's vector-Jacobian product without the Jacobians (backpropagation through time, shooting).
+ * dojo_rollout_tape is the recording rollout of dojo_rollout_grad without the Jacobians: Z_traj [13Nb x B x (T+1)] (slab 0 = Z0), the
+ * TAPE [Nres x B x T] -- the final solver iterate of every pair (t, e) at t*B + e, in the library's internal ordering (opaque; only
+ * dojo_rollout_vjp reads it) -- and status / iters [B x T] (nullable), bit for bit those of dojo_rollout_grad.  U [nu x B x T] nullable
+ * = zero input.
+ * dojo_rollout_vjp is the reverse-mode derivative of the rollout recorded by dojo_rollout_tape (same Z_traj, U, tape):
+ *   lambda_T = gZ[T];  for t = T-1 .. 0:  gU[t] = Fu_t' lambda_{t+1},  lambda_t = Fz_t' lambda_{t+1} + gZ[t];   gZ0 = lambda_0
+ * with Fz_t, Fu_t exactly the Jacobians dojo_rollout_grad returns (consistent IFT, inputs' configuration derivative included), up to
+ * rounding: one transposed solve against each step's KKT factor instead of 12Nb + nu column solves.  Cotangents are in the gradients'
+ * attitude-reduced packing [x, v, phi, w] per body: gZ [12Nb x B x (T+1)] (required), gZ0 [12Nb x B] (required), gU [nu x B x T]
+ * (nullable), status [B] (nullable): 0, or 3 if a factorisation of the backward pass was not finite (then that environment's gZ0 and gU
+ * are NaN; the others are unaffected bit for bit).  An environment's results do not depend on B, the other environments or the launch.
+ * It takes no solver options: it runs no Newton iteration.
+ * Both: B in 1..max_batch, T >= 1, the required buffers (DOJO_EINVAL otherwise, before anything is launched); DOJO_ENOMEM when the
+ * gradient workspace does not fit (as dojo_step_grad).  Host or device pointers, all of one kind (host arrays are staged through
+ * grow-only buffers of the handle); the _async forms take device pointers and do not synchronise.  Flags, external forces and the Q1 / Q2
+ * literal variants are single-step features, as for dojo_rollout_grad. */
+int dojo_rollout_tape(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const double* U, double* Z_traj,
+                      double* tape, int32_t* status, int32_t* iters);
+int dojo_rollout_tape_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZ_traj,
+                            double* dtape, int32_t* dstatus, int32_t* diters, void* cuda_stream);
+int dojo_rollout_vjp(DojoHandle* h, int B, int T, const double* Z_traj, const double* U, const double* tape, const double* gZ, double* gZ0,
+                     double* gU, int32_t* status);
+int dojo_rollout_vjp_async(DojoHandle* h, int B, int T, const double* dZ_traj, const double* dU, const double* dtape, const double* dgZ,
+                           double* dgZ0, double* dgU, int32_t* dstatus, void* cuda_stream);
 
 /* Batched environment layer (DojoEnvironments/src/environments.jl:77-109 and environments/{ant_ars,quadruped_sampling,
  * pendulum}.jl): state_map / input_map / step! / get_state plus the reward and failure test of the learning examples

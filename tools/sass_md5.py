@@ -4,9 +4,9 @@
 
 One line per kernel: md5 of its instructions as `cuobjdump -sass` prints them (text only: addresses and encodings are dropped),
 instruction count, demangled name.  Two builds whose untraced kernels print the same md5 run the same machine code; the names are
-printed demangled and trailing TRACE = false / SMALL = false / REC = false / FB = false template arguments are dropped, so that builds
-before and after the traced, the small-mechanism, the recording-rollout and the closed-loop kernels were added can be compared line by
-line (DESIGN.md section 6).
+printed demangled and trailing TRACE = false / SMALL = false / REC = false / FB = false / VJP = false template arguments are dropped, so
+that builds before and after the traced, the small-mechanism, the recording-rollout, the closed-loop and the adjoint kernels were added
+can be compared line by line (DESIGN.md section 6).
 """
 import hashlib
 import os
@@ -47,7 +47,7 @@ def main():
     ks = {n: v for n, v in kernels(lib).items() if "dojo_step_kernel" in n}
     for mangled, name in sorted(zip(ks, demangle(list(ks))), key=lambda t: t[1]):
         m = re.match(r"(.*)<(.*)>$", name)
-        if m:  # <GRAD, PLAN_SMEM[, TRACE[, SMALL[, REC[, FB]]]]>: defaulted trailing arguments are not printed
+        if m:  # <GRAD, PLAN_SMEM[, TRACE[, SMALL[, REC[, FB[, VJP]]]]]>: defaulted trailing arguments are not printed
             args = m.group(2).split(", ")
             while len(args) > 2 and args[-1] == "false":
                 args.pop()
