@@ -159,7 +159,7 @@ struct DojoHandle {
   size_t arena_bytes = 0, grad_bytes = 0;  // per environment
   size_t smem_fwd = 0, smem_grad = 0;     // dynamic shared memory per CTA
   int envs_per_sm_grad = 1;
-  double *d_Fz[2] = {nullptr, nullptr}, *d_Fu[2] = {nullptr, nullptr};  // staging for host-pointer gradient calls (grad_chunk environments, double buffered)
+  double *d_Fz[2] = {nullptr, nullptr}, *d_Fu[2] = {nullptr, nullptr};  // gradient chunk buffers (grad_chunk environments, double buffered)
   cudaEvent_t ev_kernel[2] = {nullptr, nullptr}, ev_copy[2] = {nullptr, nullptr};
   cudaStream_t copy_stream = nullptr;
   int grad_chunk = 0;
@@ -170,16 +170,13 @@ struct DojoHandle {
   int plan_smem_bytes = 0, plan_smem_bytes_grad = 0, plan_smem_mask = 0, plan_smem_mask_grad = 0;  // prefix of the blob kept in shared memory / tables inside it
   int* d_counter = nullptr;
   int* d_kin_order = nullptr;      // joints root -> leaves (minimal -> maximal map)
-  double *d_X = nullptr, *d_Xn = nullptr;  // minimal-state staging [2 nu x max_batch]
-  double *d_envTheta = nullptr, *d_envNorm = nullptr;  // policy rollout: [na x ns x max_batch], [2 ns]
-  double *d_envS = nullptr, *d_envSn = nullptr, *d_envA = nullptr, *d_envR = nullptr, *d_envS0 = nullptr;  // environment-layer staging
+  double* d_envNorm = nullptr;  // policy rollout: observation mean and standard deviation [2 ns]
+  double *d_envS = nullptr, *d_envSn = nullptr, *d_envA = nullptr, *d_envR = nullptr, *d_envS0 = nullptr;  // environment-layer scratch
   int32_t* d_envDone = nullptr;
-  double *d_recZ[2] = {nullptr, nullptr}, *d_recS = nullptr, *d_recD = nullptr;  // dojo_simulate_record staging
+  double *d_recZ[2] = {nullptr, nullptr}, *d_recS = nullptr, *d_recD = nullptr;  // dojo_simulate_record scratch
   int32_t* d_recAny = nullptr;
   double* d_kjws = nullptr;        // workspace of the map-Jacobian kernel (one slice per CTA)
   int kj_grid = 0;
-  double *d_kjout = nullptr;       // staging of map Jacobians / minimal gradients for host-pointer calls
-  size_t kjout_doubles = 0;
   int* d_done = nullptr;           // [0] finished count, [1] gradient work queue, [2..] completion-ordered environment list
   bool overlap_grad = true;
   double* d_gsol = nullptr;        // final solutions handed from the forward to the gradient launch [nres x max_batch]
@@ -190,10 +187,12 @@ struct DojoHandle {
   int lpt_mode = 1;                // 1: least-likely-to-stall last (dojo_risk_key_kernel), 2: previous call's iteration counts, 0: index order
   int32_t* d_key = nullptr;        // sort keys of the work-queue order
   unsigned long long* d_prof = nullptr;
-  // staging for host-pointer calls
+  // single-batch scratch of the environment, recording and minimal-coordinate steps, and the staging of dojo_step / dojo_step_trace
   double *d_Z = nullptr, *d_U = nullptr, *d_F = nullptr, *d_Zn = nullptr, *d_sol = nullptr;
   int32_t *d_status = nullptr, *d_iters = nullptr;
-  double *p_in = nullptr, *p_out = nullptr;  // pinned
+  double *p_in = nullptr, *p_out = nullptr;  // pinned, dojo_step / dojo_step_trace only
+  char* d_stage = nullptr;  // grow-only staging arena of the other host-pointer calls (HostCall)
+  size_t stage_bytes = 0;
   cudaStream_t stream = nullptr;
   // one call in flight per handle: the work queue counter, completion lists, staging and scratch buffers belong to the handle.
   // Calls on DIFFERENT streams are ordered behind each other through this event (enter_call / leave_call), so that an async call
@@ -201,8 +200,6 @@ struct DojoHandle {
   cudaEvent_t ev_last = nullptr;
   cudaStream_t last_stream = nullptr;
   bool has_last = false;
-  double *d_rollU = nullptr, *d_rollTraj = nullptr;  // grow-only staging of dojo_rollout (host-pointer calls)
-  size_t rollU_bytes = 0, rollTraj_bytes = 0;
   int64_t launches = 0;
   bool any_contact = false;                       // the mechanism needs the DJ_ANY_CONTACT kernels (dojo_b200_cm.cu): it has ...
   bool orthant_contact = false;                   // ... an ImpactContact / LinearContact
@@ -215,25 +212,18 @@ struct DojoHandle {
   const void* k_fwd_rec = nullptr;                 // recording rollout kernel (REC), set up by the first dojo_rollout_grad call
   int envs_per_sm_rec = 1;
   // dojo_rollout_grad scratch per (environment, step) pair, grow-only: final solutions [nres x pairs], completion list [2 + pairs]
-  // (as d_done), status and iterations [pairs]; host-pointer calls also stage the trajectory [nz x B x (T + 1)], the inputs and the
-  // minimal trajectory
+  // (as d_done), status and iterations [pairs]; the maximal trajectory [nz x B x (T + 1)] of dojo_rollout_minimal_gradients
   double* d_rsol = nullptr;
   int* d_rdone = nullptr;
   int32_t *d_rstatus = nullptr, *d_riters = nullptr;
   size_t rpairs = 0;
-  double *d_rZ = nullptr, *d_rU = nullptr, *d_rX = nullptr;
-  size_t rZ_bytes = 0, rU_bytes = 0, rX_bytes = 0;
+  double* d_rZ = nullptr;
+  size_t rZ_bytes = 0;
   const void* k_fwd_fb = nullptr;                  // closed-loop rollout kernel (FB), set up by the first dojo_rollout_feedback call
   int envs_per_sm_fb = 1;
   double* d_fbX = nullptr;                         // FB scratch: x_t [2nu x max_batch], then u_t [nu x max_batch] (no U_applied)
-  double* d_fb = nullptr;                          // grow-only staging of host-pointer dojo_rollout_feedback calls
-  size_t fb_bytes = 0;
-  double* d_lqr = nullptr;                         // grow-only staging of host-pointer dojo_lqr_backward calls
-  size_t lqr_bytes = 0;
   bool lqr_ready = false;                          // dojo_lqr_backward_kernel has the device's shared-memory maximum
   const void* k_vjp = nullptr;                     // adjoint kernel (VJP), set up by the first dojo_rollout_vjp call
-  double* d_vjp = nullptr;                         // grow-only staging of host-pointer dojo_rollout_tape / dojo_rollout_vjp calls
-  size_t vjp_bytes = 0;
   std::string err;
 };
 // Whether the forward kernel specialised for small mechanisms (dojo_step_kernel.cuh, SMALL) computes this handle's step exactly: the
@@ -815,7 +805,7 @@ extern "C" int dojo_create(const DojoMechanismDesc* d, int device, int max_batch
 extern "C" int dojo_destroy(DojoHandle* h) {
   if (!h) return DOJO_OK;
   cudaSetDevice(h->device);
-  cudaFree(h->d_key); cudaFree(h->d_order); cudaFree(h->d_prev_iters); cudaFree(h->d_prof); cudaFree(h->d_blob); cudaFree(h->d_counter); cudaFree(h->d_kin_order); cudaFree(h->d_kjws); cudaFree(h->d_kjout); cudaFree(h->d_recZ[0]); cudaFree(h->d_recZ[1]); cudaFree(h->d_recS); cudaFree(h->d_recD); cudaFree(h->d_recAny); cudaFree(h->d_envTheta); cudaFree(h->d_envNorm); cudaFree(h->d_envS); cudaFree(h->d_envSn); cudaFree(h->d_envA); cudaFree(h->d_envR); cudaFree(h->d_envS0); cudaFree(h->d_envDone); cudaFree(h->d_X); cudaFree(h->d_Xn); cudaFree(h->d_gsol); cudaFree(h->d_gstatus); cudaFree(h->d_done); cudaFree(h->d_trace);
+  cudaFree(h->d_key); cudaFree(h->d_order); cudaFree(h->d_prev_iters); cudaFree(h->d_prof); cudaFree(h->d_blob); cudaFree(h->d_counter); cudaFree(h->d_kin_order); cudaFree(h->d_kjws); cudaFree(h->d_recZ[0]); cudaFree(h->d_recZ[1]); cudaFree(h->d_recS); cudaFree(h->d_recD); cudaFree(h->d_recAny); cudaFree(h->d_envNorm); cudaFree(h->d_envS); cudaFree(h->d_envSn); cudaFree(h->d_envA); cudaFree(h->d_envR); cudaFree(h->d_envS0); cudaFree(h->d_envDone); cudaFree(h->d_gsol); cudaFree(h->d_gstatus); cudaFree(h->d_done); cudaFree(h->d_trace);
   for (int k = 0; k < 2; ++k) { cudaFree(h->d_Fz[k]); cudaFree(h->d_Fu[k]); if (h->ev_kernel[k]) cudaEventDestroy(h->ev_kernel[k]); if (h->ev_copy[k]) cudaEventDestroy(h->ev_copy[k]); }
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
   cudaFree(h->d_Z); cudaFree(h->d_U); cudaFree(h->d_F); cudaFree(h->d_Zn); cudaFree(h->d_sol); cudaFree(h->d_status); cudaFree(h->d_iters);
@@ -823,9 +813,9 @@ extern "C" int dojo_destroy(DojoHandle* h) {
   if (h->p_out) cudaFreeHost(h->p_out);
   if (h->stream) cudaStreamDestroy(h->stream);
   if (h->ev_last) cudaEventDestroy(h->ev_last);
-  cudaFree(h->d_rollU); cudaFree(h->d_rollTraj);
-  cudaFree(h->d_rsol); cudaFree(h->d_rdone); cudaFree(h->d_rstatus); cudaFree(h->d_riters); cudaFree(h->d_rZ); cudaFree(h->d_rU); cudaFree(h->d_rX);
-  cudaFree(h->d_fbX); cudaFree(h->d_fb); cudaFree(h->d_lqr);
+  cudaFree(h->d_stage);
+  cudaFree(h->d_rsol); cudaFree(h->d_rdone); cudaFree(h->d_rstatus); cudaFree(h->d_riters); cudaFree(h->d_rZ);
+  cudaFree(h->d_fbX);
   delete h;
   return DOJO_OK;
 }
@@ -951,6 +941,60 @@ static bool is_pinned_host_ptr(const void* p) {
   return at.type == cudaMemoryTypeHost;
 }
 
+// grow-only device buffer; a buffer that is replaced may still be read by the handle's last call
+static int grow_buffer(DojoHandle* h, void** buf, size_t* have, size_t need) {
+  if (*have >= need) return DOJO_OK;
+  CUDA_TRY(h, cudaDeviceSynchronize());
+  cudaFree(*buf); *buf = nullptr; *have = 0;
+  CUDA_TRY(h, cudaMalloc(buf, need));
+  *have = need;
+  return DOJO_OK;
+}
+
+// The arrays of one synchronous host- or device-pointer entry (every entry but dojo_step / dojo_step_trace).  The pointer kind is
+// decided once, from the call's first array; the others are of the same kind.  Device pointers pass through.  With host pointers each
+// declared array gets a 256-byte aligned slice of the handle's grow-only staging arena (a null or empty array gets none, and a null
+// pointer): bind() points the caller's variables at the slices and copies the inputs in, finish() copies the non-null outputs out, both
+// on h->stream and straight from / to the caller's buffers.  finish() ends the call with one synchronisation in either case.
+struct HostCall {
+  enum { IN = 1, OUT = 2, SCRATCH = 4 };
+  struct Array { void* var; const void* host; size_t bytes; int use; size_t off; };
+  DojoHandle* h;
+  bool dev;
+  std::vector<Array> arrays;
+  HostCall(DojoHandle* h, const void* first) : h(h), dev(is_device_ptr(first)) {}
+  // *p holds the caller's array of n elements; scratch: device memory of host-pointer calls only
+  template <class T> void in(T** p, size_t n) { arrays.push_back({(void*)p, (const void*)*p, n * sizeof(T), IN, 0}); }
+  template <class T> void out(T** p, size_t n) { arrays.push_back({(void*)p, (const void*)*p, n * sizeof(T), OUT, 0}); }
+  template <class T> void inout(T** p, size_t n) { arrays.push_back({(void*)p, (const void*)*p, n * sizeof(T), IN | OUT, 0}); }
+  template <class T> void scratch(T** p, size_t n) { arrays.push_back({(void*)p, nullptr, n * sizeof(T), SCRATCH, 0}); }
+  int bind() {
+    if (dev) return DOJO_OK;
+    size_t total = 0;
+    for (Array& a : arrays) {
+      if (!a.host && a.use != SCRATCH) a.bytes = 0;
+      a.off = total;
+      total += (a.bytes + 255) & ~size_t(255);
+    }
+    int rc = grow_buffer(h, (void**)&h->d_stage, &h->stage_bytes, total);
+    if (rc != DOJO_OK) return rc;
+    for (Array& a : arrays) {
+      char* d = a.bytes ? h->d_stage + a.off : nullptr;
+      std::memcpy(a.var, &d, sizeof(d));  // the caller's T* variable now points at the slice
+      if (a.bytes && (a.use & IN)) CUDA_TRY(h, cudaMemcpyAsync(d, a.host, a.bytes, cudaMemcpyHostToDevice, h->stream));
+    }
+    return DOJO_OK;
+  }
+  // rc: the entry's result so far; an error is returned as it is
+  int finish(int rc = DOJO_OK) {
+    if (rc != DOJO_OK) return rc;
+    for (const Array& a : arrays)
+      if (!dev && a.bytes && (a.use & OUT)) CUDA_TRY(h, cudaMemcpyAsync((void*)a.host, h->d_stage + a.off, a.bytes, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    return DOJO_OK;
+  }
+};
+
 static int ensure_staging(DojoHandle* h) {
   if (h->d_Z) return DOJO_OK;
   const Plan& P = h->plan;
@@ -962,8 +1006,6 @@ static int ensure_staging(DojoHandle* h) {
   CUDA_TRY(h, cudaMalloc((void**)&h->d_sol, B * P.nres * sizeof(double)));
   CUDA_TRY(h, cudaMalloc((void**)&h->d_status, B * sizeof(int32_t)));
   CUDA_TRY(h, cudaMalloc((void**)&h->d_iters, B * sizeof(int32_t)));
-  CUDA_TRY(h, cudaMalloc((void**)&h->d_X, std::max<size_t>(1, B * 2 * P.nu) * sizeof(double)));
-  CUDA_TRY(h, cudaMalloc((void**)&h->d_Xn, std::max<size_t>(1, B * 2 * P.nu) * sizeof(double)));
   CUDA_TRY(h, cudaMallocHost((void**)&h->p_in, B * (P.nz + P.nu + 6 * P.Nb) * sizeof(double)));
   CUDA_TRY(h, cudaMallocHost((void**)&h->p_out, B * (P.nz + P.nres + 2) * sizeof(double)));
   return DOJO_OK;
@@ -1098,37 +1140,15 @@ extern "C" int dojo_rollout(DojoHandle* h, const DojoSolverOptions* opts, int B,
                             int32_t* status_any) {
   if (!h || B <= 0 || B > h->max_batch || T <= 0 || !Z0 || !Z_final) { if (h) h->err = "dojo_rollout: bad arguments"; return DOJO_EINVAL; }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = h->stream;
-  if (is_device_ptr(Z0)) {
-    int rc = launch_rollout(h, opts, B, T, Z0, U, Z_final, Z_traj, status_any, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
-  int rc = ensure_staging(h);
-  if (rc != DOJO_OK) return rc;
-  const Plan& P = h->plan;
-  const size_t zbytes = (size_t)B * P.nz * sizeof(double), ubytes = (size_t)B * P.nu * sizeof(double) * T;
-  double *dU = nullptr, *dtraj = nullptr;
-  auto grow = [&](double** buf, size_t* have, size_t need) -> cudaError_t {  // grow-only: no allocation in steady state
-    if (*have >= need) return cudaSuccess;
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) return e;
-    cudaFree(*buf); *buf = nullptr; *have = 0;
-    e = cudaMalloc((void**)buf, need);
-    if (e == cudaSuccess) *have = need;
-    return e;
-  };
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_Z, Z0, zbytes, cudaMemcpyHostToDevice, s));
-  if (U && P.nu > 0) { CUDA_TRY(h, grow(&h->d_rollU, &h->rollU_bytes, ubytes)); dU = h->d_rollU; CUDA_TRY(h, cudaMemcpyAsync(dU, U, ubytes, cudaMemcpyHostToDevice, s)); }
-  if (Z_traj) { CUDA_TRY(h, grow(&h->d_rollTraj, &h->rollTraj_bytes, zbytes * T)); dtraj = h->d_rollTraj; }
-  rc = launch_rollout(h, opts, B, T, h->d_Z, dU, h->d_Zn, dtraj, h->d_status, s);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(Z_final, h->d_Zn, zbytes, cudaMemcpyDeviceToHost, s));
-  if (Z_traj) CUDA_TRY(h, cudaMemcpyAsync(Z_traj, dtraj, zbytes * T, cudaMemcpyDeviceToHost, s));
-  if (status_any) CUDA_TRY(h, cudaMemcpyAsync(status_any, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  const size_t nz = (size_t)B * h->plan.nz;
+  const double *dZ0 = Z0, *dU = U;
+  double *dZf = Z_final, *dtraj = Z_traj;
+  int32_t* dst = status_any;
+  HostCall c(h, Z0);
+  c.in(&dZ0, nz); c.in(&dU, (size_t)B * h->plan.nu * T); c.out(&dZf, nz); c.out(&dtraj, nz * T); c.out(&dst, B);
+  int rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_rollout(h, opts, B, T, dZ0, dU, dZf, dtraj, dst, h->stream);
+  return c.finish(rc);
 }
 
 // gradients: implemented in dojo_grad.cu
@@ -1322,47 +1342,52 @@ static int ensure_grad_chunks(DojoHandle* h) {
   return DOJO_OK;
 }
 
+// Jacobians of `count` environments or pairs to the host through the two chunk buffers: launch(i0, n, k) computes items [i0, i0 + n)
+// into d_Fz[k] / d_Fu[k] on h->stream, and their copies to Fz / Fu (fz / fu doubles per item) run on copy_stream while the next chunk
+// is computed.  The caller synchronises copy_stream.
+template <class Launch>
+static int copy_out_chunks(DojoHandle* h, size_t count, double* Fz, size_t fz, double* Fu, size_t fu, Launch launch) {
+  cudaStream_t s = h->stream, cs = h->copy_stream;
+  int k = 0;
+  for (size_t i0 = 0; i0 < count; i0 += h->grad_chunk, k ^= 1) {
+    const int n = (int)std::min<size_t>(h->grad_chunk, count - i0);
+    if (i0 >= 2 * (size_t)h->grad_chunk) CUDA_TRY(h, cudaStreamWaitEvent(s, h->ev_copy[k], 0));  // buffer k has been drained
+    int rc = launch(i0, n, k);
+    if (rc != DOJO_OK) return rc;
+    CUDA_TRY(h, cudaEventRecord(h->ev_kernel[k], s));
+    CUDA_TRY(h, cudaStreamWaitEvent(cs, h->ev_kernel[k], 0));
+    CUDA_TRY(h, cudaMemcpyAsync(Fz + i0 * fz, h->d_Fz[k], (size_t)n * fz * sizeof(double), cudaMemcpyDeviceToHost, cs));
+    if (fu) CUDA_TRY(h, cudaMemcpyAsync(Fu + i0 * fu, h->d_Fu[k], (size_t)n * fu * sizeof(double), cudaMemcpyDeviceToHost, cs));
+    CUDA_TRY(h, cudaEventRecord(h->ev_copy[k], cs));
+  }
+  return DOJO_OK;
+}
+
 // Host- or device-pointer entry.  Host buffers are processed in chunks (the Jacobians are large: (12Nb)^2 doubles per env).
 extern "C" int dojo_step_grad(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* Z, const double* U, const double* Fext, double* Zn,
                               double* Fz, double* Fu, int32_t* status, int32_t* iters, uint32_t flags) {
   if (!h || B <= 0 || B > h->max_batch || !Z || !Zn || !Fz || !Fu) { if (h) h->err = "dojo_step_grad: bad arguments"; return DOJO_EINVAL; }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  const Plan& P = h->plan;
-  if (is_device_ptr(Z)) {
-    int rc = dojo_step_grad_async(h, opts, B, Z, U, Fext, Zn, Fz, Fu, status, iters, flags, h->stream);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    return DOJO_OK;
-  }
-  int rc = ensure_staging(h);
-  if (rc == DOJO_OK) rc = ensure_grad_chunks(h);
+  HostCall c(h, Z);
+  if (c.dev) return c.finish(dojo_step_grad_async(h, opts, B, Z, U, Fext, Zn, Fz, Fu, status, iters, flags, h->stream));
+  int rc = ensure_grad_chunks(h);
   if (rc != DOJO_OK) return rc;
+  const Plan& P = h->plan;
   const size_t ng = 12 * (size_t)P.Nb, fz = ng * ng, fu = ng * P.nu;
-  cudaStream_t s = h->stream, cs = h->copy_stream;
   // whole-batch inputs first (small), per-chunk kernels, gradient copies on the second stream
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_Z, Z, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
-  if (U && P.nu > 0) CUDA_TRY(h, cudaMemcpyAsync(h->d_U, U, (size_t)B * P.nu * sizeof(double), cudaMemcpyHostToDevice, s));
-  if (Fext) CUDA_TRY(h, cudaMemcpyAsync(h->d_F, Fext, (size_t)B * 6 * P.Nb * sizeof(double), cudaMemcpyHostToDevice, s));
-  int k = 0;
-  for (int e0 = 0; e0 < B; e0 += h->grad_chunk, k ^= 1) {
-    const int nb = std::min(h->grad_chunk, B - e0);
-    if (e0 >= 2 * h->grad_chunk) CUDA_TRY(h, cudaStreamWaitEvent(s, h->ev_copy[k], 0));  // buffer k has been drained
-    rc = dojo_step_grad_async(h, opts, nb, h->d_Z + (size_t)e0 * P.nz, (U && P.nu > 0) ? h->d_U + (size_t)e0 * P.nu : nullptr,
-                              Fext ? h->d_F + (size_t)e0 * 6 * P.Nb : nullptr, h->d_Zn + (size_t)e0 * P.nz, h->d_Fz[k], h->d_Fu[k], h->d_status + e0,
-                              h->d_iters + e0, flags, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaEventRecord(h->ev_kernel[k], s));
-    CUDA_TRY(h, cudaStreamWaitEvent(cs, h->ev_kernel[k], 0));
-    CUDA_TRY(h, cudaMemcpyAsync(Fz + (size_t)e0 * fz, h->d_Fz[k], (size_t)nb * fz * sizeof(double), cudaMemcpyDeviceToHost, cs));
-    if (fu) CUDA_TRY(h, cudaMemcpyAsync(Fu + (size_t)e0 * fu, h->d_Fu[k], (size_t)nb * fu * sizeof(double), cudaMemcpyDeviceToHost, cs));
-    CUDA_TRY(h, cudaEventRecord(h->ev_copy[k], cs));
-  }
-  CUDA_TRY(h, cudaMemcpyAsync(Zn, h->d_Zn, (size_t)B * P.nz * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  CUDA_TRY(h, cudaStreamSynchronize(cs));
-  return DOJO_OK;
+  const double *dZ = Z, *dU = U, *dF = Fext;
+  double* dZn = Zn;
+  int32_t *dst = status, *dit = iters;
+  c.in(&dZ, (size_t)B * P.nz); c.in(&dU, (size_t)B * P.nu); c.in(&dF, (size_t)B * 6 * P.Nb);
+  c.out(&dZn, (size_t)B * P.nz); c.out(&dst, B); c.out(&dit, B);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = copy_out_chunks(h, B, Fz, fz, Fu, fu, [&](size_t e0, int nb, int k) {
+    return dojo_step_grad_async(h, opts, nb, dZ + e0 * P.nz, dU ? dU + e0 * P.nu : nullptr, dF ? dF + e0 * 6 * P.Nb : nullptr, dZn + e0 * P.nz,
+                                h->d_Fz[k], h->d_Fu[k], dst ? dst + e0 : nullptr, dit ? dit + e0 : nullptr, flags, h->stream);
+  });
+  rc = c.finish(rc);
+  if (rc == DOJO_OK) CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));
+  return rc;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1398,25 +1423,14 @@ extern "C" int dojo_maximal_to_minimal_async(DojoHandle* h, int B, const double*
 static int kin_sync(DojoHandle* h, bool to_maximal, int B, const double* in, double* out, const char* who) {
   if (!h || B <= 0 || B > h->max_batch || !in || !out) { if (h) h->err = std::string(who) + ": bad arguments"; return DOJO_EINVAL; }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  const Plan& P = h->plan;
-  cudaStream_t s = h->stream;
-  const size_t nx = (size_t)B * 2 * P.nu * sizeof(double), nzb = (size_t)B * P.nz * sizeof(double);
-  if (is_device_ptr(in)) {
-    int rc = launch_kin(h, to_maximal, B, in, out, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
-  int rc = ensure_staging(h);
-  if (rc != DOJO_OK) return rc;
-  double* din = to_maximal ? h->d_X : h->d_Z;
-  double* dout = to_maximal ? h->d_Z : h->d_X;
-  CUDA_TRY(h, cudaMemcpyAsync(din, in, to_maximal ? nx : nzb, cudaMemcpyHostToDevice, s));
-  rc = launch_kin(h, to_maximal, B, din, dout, s);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(out, dout, to_maximal ? nzb : nx, cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  const size_t nx = (size_t)B * 2 * h->plan.nu, nz = (size_t)B * h->plan.nz;
+  const double* din = in;
+  double* dout = out;
+  HostCall c(h, in);
+  c.in(&din, to_maximal ? nx : nz); c.out(&dout, to_maximal ? nz : nx);
+  int rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_kin(h, to_maximal, B, din, dout, h->stream);
+  return c.finish(rc);
 }
 extern "C" int dojo_minimal_to_maximal(DojoHandle* h, int B, const double* X, double* Z) { return kin_sync(h, true, B, X, Z, "dojo_minimal_to_maximal"); }
 extern "C" int dojo_maximal_to_minimal(DojoHandle* h, int B, const double* Z, double* X) { return kin_sync(h, false, B, Z, X, "dojo_maximal_to_minimal"); }
@@ -1437,28 +1451,17 @@ extern "C" int dojo_step_minimal_flags(DojoHandle* h, const DojoSolverOptions* o
   if (rc != DOJO_OK) return rc;
   const Plan& P = h->plan;
   cudaStream_t s = h->stream;
-  const bool dev = is_device_ptr(X);
-  const size_t nx = (size_t)B * 2 * P.nu * sizeof(double);
-  const double* dX = X;
-  const double* dU = U;
+  const size_t nx = (size_t)B * 2 * P.nu;
+  const double *dX = X, *dU = U;
   double* dXn = X_next;
-  if (!dev) {
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_X, X, nx, cudaMemcpyHostToDevice, s));
-    if (U && P.nu > 0) CUDA_TRY(h, cudaMemcpyAsync(h->d_U, U, (size_t)B * P.nu * sizeof(double), cudaMemcpyHostToDevice, s));
-    dX = h->d_X; dU = (U && P.nu > 0) ? h->d_U : nullptr; dXn = h->d_Xn;
-  }
-  rc = launch_kin(h, true, B, dX, h->d_Z, s);
-  if (rc == DOJO_OK) rc = launch_forward(h, opts, B, h->d_Z, dU, nullptr, h->d_Zn, nullptr, nullptr, dev ? status : h->d_status, dev ? iters : h->d_iters,
-                                            flags & DOJO_FLAG_Q1_LITERAL_RETURN, s);
+  int32_t *dst = status, *dit = iters;
+  HostCall c(h, X);
+  c.in(&dX, nx); c.in(&dU, (size_t)B * P.nu); c.out(&dXn, nx); c.out(&dst, B); c.out(&dit, B);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_kin(h, true, B, dX, h->d_Z, s);
+  if (rc == DOJO_OK) rc = launch_forward(h, opts, B, h->d_Z, dU, nullptr, h->d_Zn, nullptr, nullptr, dst, dit, flags & DOJO_FLAG_Q1_LITERAL_RETURN, s);
   if (rc == DOJO_OK) rc = launch_kin(h, false, B, h->d_Zn, dXn, s);
-  if (rc != DOJO_OK) return rc;
-  if (!dev) {
-    CUDA_TRY(h, cudaMemcpyAsync(X_next, h->d_Xn, nx, cudaMemcpyDeviceToHost, s));
-    if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  }
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  return c.finish(rc);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1468,13 +1471,6 @@ static int ensure_kinjac(DojoHandle* h) {
   if (h->d_kjws) return DOJO_OK;
   h->kj_grid = std::max(1, std::min(h->max_batch, h->sm_count * 4));  // 254 registers x 128 threads: two CTAs resident per SM
   CUDA_TRY(h, cudaMalloc((void**)&h->d_kjws, (size_t)h->kj_grid * kinjac_ws_doubles(h->plan.Nb, h->plan.nu) * sizeof(double)));
-  return DOJO_OK;
-}
-static int ensure_kjout(DojoHandle* h, size_t doubles) {
-  if (h->kjout_doubles >= doubles) return DOJO_OK;
-  if (h->d_kjout) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(h->d_kjout); h->d_kjout = nullptr; h->kjout_doubles = 0; }
-  CUDA_TRY(h, cudaMalloc((void**)&h->d_kjout, doubles * sizeof(double)));
-  h->kjout_doubles = doubles;
   return DOJO_OK;
 }
 
@@ -1516,27 +1512,20 @@ static int kinjac_sync(DojoHandle* h, int mode, int B, const double* Z, double* 
   CUDA_TRY(h, cudaSetDevice(h->device));
   const Plan& P = h->plan;
   cudaStream_t s = h->stream;
-  if (is_device_ptr(Z)) {
-    int rc = launch_kinjac(h, mode, B, Z, nullptr, nullptr, nullptr, J, nullptr, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
-  int rc = ensure_staging(h);
-  if (rc != DOJO_OK) return rc;
+  HostCall c(h, Z);
+  if (c.dev) return c.finish(launch_kinjac(h, mode, B, Z, nullptr, nullptr, nullptr, J, nullptr, s));
   const size_t per_env = (size_t)2 * P.nu * 12 * P.Nb;
   const int chunk = (int)std::max<size_t>(1, std::min<size_t>(B, (size_t(256) << 20) / std::max<size_t>(1, per_env * sizeof(double))));
-  rc = ensure_kjout(h, (size_t)chunk * per_env);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_Z, Z, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
-  for (int e0 = 0; e0 < B; e0 += chunk) {
+  const double* dZ = Z;
+  double* dJ = nullptr;
+  c.in(&dZ, (size_t)B * P.nz); c.scratch(&dJ, (size_t)chunk * per_env);
+  int rc = c.bind();
+  for (int e0 = 0; e0 < B && rc == DOJO_OK; e0 += chunk) {
     const int nb = std::min(chunk, B - e0);
-    rc = launch_kinjac(h, mode, nb, h->d_Z + (size_t)e0 * P.nz, nullptr, nullptr, nullptr, h->d_kjout, nullptr, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaMemcpyAsync(J + (size_t)e0 * per_env, h->d_kjout, (size_t)nb * per_env * sizeof(double), cudaMemcpyDeviceToHost, s));
+    rc = launch_kinjac(h, mode, nb, dZ + (size_t)e0 * P.nz, nullptr, nullptr, nullptr, dJ, nullptr, s);
+    if (rc == DOJO_OK) CUDA_TRY(h, cudaMemcpyAsync(J + (size_t)e0 * per_env, dJ, (size_t)nb * per_env * sizeof(double), cudaMemcpyDeviceToHost, s));
   }
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  return c.finish(rc);
 }
 extern "C" int dojo_maximal_to_minimal_jacobian(DojoHandle* h, int B, const double* Z, double* J) { return kinjac_sync(h, 0, B, Z, J, "dojo_maximal_to_minimal_jacobian"); }
 extern "C" int dojo_minimal_to_maximal_jacobian(DojoHandle* h, int B, const double* Z, double* J) { return kinjac_sync(h, 1, B, Z, J, "dojo_minimal_to_maximal_jacobian"); }
@@ -1548,46 +1537,29 @@ extern "C" int dojo_minimal_gradients(DojoHandle* h, const DojoSolverOptions* op
   if (!h || B <= 0 || B > h->max_batch || !X || !X_next || !Gx || !Gu) { if (h) h->err = "dojo_minimal_gradients: bad arguments"; return DOJO_EINVAL; }
   CUDA_TRY(h, cudaSetDevice(h->device));
   int rc = ensure_staging(h);
+  if (rc == DOJO_OK) rc = ensure_grad_chunks(h);  // same chunk buffers as the host-pointer path of dojo_step_grad
   if (rc != DOJO_OK) return rc;
   const Plan& P = h->plan;
   cudaStream_t s = h->stream;
-  const bool dev = is_device_ptr(X);
   const size_t nm = 2 * (size_t)P.nu, gx = nm * nm, gu = nm * P.nu;
-  rc = ensure_grad_chunks(h);  // same chunk buffers as the host-pointer path of dojo_step_grad
-  if (rc != DOJO_OK) return rc;
-  const double* dX = X;
-  const double* dU = (U && P.nu > 0) ? U : nullptr;
+  const double *dX = X, *dU = (U && P.nu > 0) ? U : nullptr;
   double *dXn = X_next, *dGx = Gx, *dGu = Gu;
   int32_t *dst = status, *dit = iters;
-  if (!dev) {
-    rc = ensure_kjout(h, (size_t)B * (gx + gu));
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_X, X, (size_t)B * nm * sizeof(double), cudaMemcpyHostToDevice, s));
-    if (dU) { CUDA_TRY(h, cudaMemcpyAsync(h->d_U, U, (size_t)B * P.nu * sizeof(double), cudaMemcpyHostToDevice, s)); dU = h->d_U; }
-    dX = h->d_X; dXn = h->d_Xn; dGx = h->d_kjout; dGu = h->d_kjout + (size_t)B * gx; dst = h->d_status; dit = h->d_iters;
-  }
-  rc = launch_kin(h, true, B, dX, h->d_Z, s);
-  if (rc != DOJO_OK) return rc;
-  for (int e0 = 0; e0 < B; e0 += h->grad_chunk) {
+  HostCall c(h, X);
+  c.in(&dX, B * nm); c.in(&dU, (size_t)B * P.nu);
+  c.out(&dXn, B * nm); c.out(&dGx, B * gx); c.out(&dGu, B * gu); c.out(&dst, B); c.out(&dit, B);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_kin(h, true, B, dX, h->d_Z, s);
+  for (int e0 = 0; e0 < B && rc == DOJO_OK; e0 += h->grad_chunk) {
     const int nb = std::min(h->grad_chunk, B - e0);
     rc = dojo_step_grad_async(h, opts, nb, h->d_Z + (size_t)e0 * P.nz, dU ? dU + (size_t)e0 * P.nu : nullptr, nullptr, h->d_Zn + (size_t)e0 * P.nz,
                               h->d_Fz[0], h->d_Fu[0], dst ? dst + e0 : nullptr, dit ? dit + e0 : nullptr, 0, s);
     if (rc == DOJO_OK)
       rc = launch_kinjac(h, 2, nb, h->d_Z + (size_t)e0 * P.nz, h->d_Zn + (size_t)e0 * P.nz, h->d_Fz[0], h->d_Fu[0], dGx + (size_t)e0 * gx,
                          dGu + (size_t)e0 * gu, s);
-    if (rc != DOJO_OK) return rc;
   }
-  rc = launch_kin(h, false, B, h->d_Zn, dXn, s);
-  if (rc != DOJO_OK) return rc;
-  if (!dev) {
-    CUDA_TRY(h, cudaMemcpyAsync(X_next, h->d_Xn, (size_t)B * nm * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(h, cudaMemcpyAsync(Gx, dGx, (size_t)B * gx * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (gu) CUDA_TRY(h, cudaMemcpyAsync(Gu, dGu, (size_t)B * gu * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  }
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  if (rc == DOJO_OK) rc = launch_kin(h, false, B, h->d_Zn, dXn, s);
+  return c.finish(rc);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1607,16 +1579,6 @@ static int ensure_rec_kernel(DojoHandle* h) {
   return DOJO_OK;
 }
 
-// grow-only device buffer; a buffer that is replaced may still be read by the handle's last call
-static int grow_buffer(DojoHandle* h, void** buf, size_t* have, size_t need) {
-  if (*have >= need) return DOJO_OK;
-  CUDA_TRY(h, cudaDeviceSynchronize());
-  cudaFree(*buf); *buf = nullptr; *have = 0;
-  CUDA_TRY(h, cudaMalloc(buf, need));
-  *have = need;
-  return DOJO_OK;
-}
-
 static int ensure_rollout_grad_scratch(DojoHandle* h, size_t pairs) {
   if (h->rpairs >= pairs) return DOJO_OK;
   CUDA_TRY(h, cudaDeviceSynchronize());
@@ -1630,23 +1592,25 @@ static int ensure_rollout_grad_scratch(DojoHandle* h, size_t pairs) {
   return DOJO_OK;
 }
 
-// argument checks and set-up shared by the three entries: no launch before every check has passed
-static int rollout_grad_setup(DojoHandle* h, int B, int T, bool buffers, const char* who) {
+// argument checks shared by the trajectory-gradient, tape and adjoint entries: no launch before every check has passed; `required`
+// names the buffers the entry needs
+static int trajectory_setup(DojoHandle* h, int B, int T, bool buffers, const char* who, const char* required) {
   if (!h) return DOJO_EINVAL;
   if (B <= 0 || B > h->max_batch || T <= 0 || !buffers || (long long)B * (T + 1) > (long long)INT_MAX - 2) {
-    h->err = std::string(who) + ": bad arguments (B in 1..max_batch, T >= 1, B * (T + 1) < 2^31 - 2, state / trajectory / Jacobian buffers required)";
+    h->err = std::string(who) + ": bad arguments (B in 1..max_batch, T >= 1, B * (T + 1) < 2^31 - 2, " + required + ")";
     return DOJO_EINVAL;
   }
   if (!h->grad_bytes) { h->err = std::string(who) + ": the gradient workspace does not fit in shared memory for this mechanism"; return DOJO_ENOMEM; }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  int rc = ensure_rec_kernel(h);
-  if (rc == DOJO_OK) rc = ensure_rollout_grad_scratch(h, (size_t)B * T);
-  return rc;
+  return DOJO_OK;
 }
+static const char* kRollGradBuffers = "state / trajectory / Jacobian buffers required";
 
 extern "C" int dojo_rollout_grad_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZ_traj,
                                        double* dFz, double* dFu, int32_t* dstatus, int32_t* diters, void* cuda_stream) {
-  int rc = rollout_grad_setup(h, B, T, dZ0 && dZ_traj && dFz && dFu, "dojo_rollout_grad_async");
+  int rc = trajectory_setup(h, B, T, dZ0 && dZ_traj && dFz && dFu, "dojo_rollout_grad_async", kRollGradBuffers);
+  if (rc == DOJO_OK) rc = ensure_rec_kernel(h);
+  if (rc == DOJO_OK) rc = ensure_rollout_grad_scratch(h, (size_t)B * T);
   if (rc != DOJO_OK) return rc;
   const Plan& P = h->plan;
   cudaStream_t s = (cudaStream_t)cuda_stream;
@@ -1668,48 +1632,36 @@ extern "C" int dojo_rollout_grad_async(DojoHandle* h, const DojoSolverOptions* o
 // two chunk buffers of dojo_step_grad, after one rollout; the gradient kernel of chunk i + 1 runs while chunk i is being copied.
 extern "C" int dojo_rollout_grad(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const double* U, double* Z_traj,
                                  double* Fz, double* Fu, int32_t* status, int32_t* iters) {
-  int rc = rollout_grad_setup(h, B, T, Z0 && Z_traj && Fz && Fu, "dojo_rollout_grad");
+  int rc = trajectory_setup(h, B, T, Z0 && Z_traj && Fz && Fu, "dojo_rollout_grad", kRollGradBuffers);
+  if (rc == DOJO_OK) rc = ensure_rec_kernel(h);
+  if (rc == DOJO_OK) rc = ensure_rollout_grad_scratch(h, (size_t)B * T);
   if (rc != DOJO_OK) return rc;
-  if (is_device_ptr(Z0)) {
-    rc = dojo_rollout_grad_async(h, opts, B, T, Z0, U, Z_traj, Fz, Fu, status, iters, h->stream);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    return DOJO_OK;
-  }
+  HostCall c(h, Z0);
+  if (c.dev) return c.finish(dojo_rollout_grad_async(h, opts, B, T, Z0, U, Z_traj, Fz, Fu, status, iters, h->stream));
   rc = ensure_grad_chunks(h);
+  if (rc != DOJO_OK) return rc;
   const Plan& P = h->plan;
   const size_t pairs = (size_t)B * T, ng = 12 * (size_t)P.Nb, fz = ng * ng, fu = ng * P.nu;
-  const bool has_u = U && P.nu > 0;
-  if (rc == DOJO_OK) rc = grow_buffer(h, (void**)&h->d_rZ, &h->rZ_bytes, (pairs + B) * P.nz * sizeof(double));
-  if (rc == DOJO_OK && has_u) rc = grow_buffer(h, (void**)&h->d_rU, &h->rU_bytes, pairs * P.nu * sizeof(double));
+  cudaStream_t s = h->stream;
+  const double* dU = U;
+  double* dtraj = Z_traj;
+  int32_t *dst = status, *dit = iters;
+  c.in(&dU, pairs * P.nu); c.out(&dtraj, (pairs + B) * P.nz); c.out(&dst, pairs); c.out(&dit, pairs);
+  rc = c.bind();
   if (rc != DOJO_OK) return rc;
-  cudaStream_t s = h->stream, cs = h->copy_stream;
-  const double* dU = has_u ? h->d_rU : nullptr;
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_rZ, Z0, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
-  if (has_u) CUDA_TRY(h, cudaMemcpyAsync(h->d_rU, U, pairs * P.nu * sizeof(double), cudaMemcpyHostToDevice, s));
-  rc = launch_rollout(h, opts, B, T, h->d_rZ, dU, nullptr, h->d_rZ + (size_t)B * P.nz, h->d_rstatus, s, h->d_riters, h->d_rsol);
-  if (rc != DOJO_OK) return rc;
-  int k = 0;
-  for (size_t p0 = 0; p0 < pairs; p0 += h->grad_chunk, k ^= 1) {
-    const int n = (int)std::min<size_t>(h->grad_chunk, pairs - p0);
-    if (p0 >= 2 * (size_t)h->grad_chunk) CUDA_TRY(h, cudaStreamWaitEvent(s, h->ev_copy[k], 0));  // buffer k has been drained
+  int32_t* st = dst ? dst : h->d_rstatus;  // the REC kernel always writes a status
+  CUDA_TRY(h, cudaMemcpyAsync(dtraj, Z0, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
+  rc = launch_rollout(h, opts, B, T, dtraj, dU, nullptr, dtraj + (size_t)B * P.nz, st, s, dit, h->d_rsol);
+  if (rc == DOJO_OK) rc = copy_out_chunks(h, pairs, Fz, fz, Fu, fu, [&](size_t p0, int n, int k) {
     enter_call(h, s);
-    rc = launch_grad(h, opts, n, h->d_rZ + p0 * P.nz, dU ? dU + p0 * P.nu : nullptr, nullptr, h->d_rsol + p0 * P.nres, h->d_rstatus + p0, h->d_Fz[k],
-                     h->d_Fu[k], nullptr, 0, nullptr, nullptr, s);
-    if (rc != DOJO_OK) return rc;
-    leave_call(h, s);
-    CUDA_TRY(h, cudaEventRecord(h->ev_kernel[k], s));
-    CUDA_TRY(h, cudaStreamWaitEvent(cs, h->ev_kernel[k], 0));
-    CUDA_TRY(h, cudaMemcpyAsync(Fz + p0 * fz, h->d_Fz[k], (size_t)n * fz * sizeof(double), cudaMemcpyDeviceToHost, cs));
-    if (fu) CUDA_TRY(h, cudaMemcpyAsync(Fu + p0 * fu, h->d_Fu[k], (size_t)n * fu * sizeof(double), cudaMemcpyDeviceToHost, cs));
-    CUDA_TRY(h, cudaEventRecord(h->ev_copy[k], cs));
-  }
-  CUDA_TRY(h, cudaMemcpyAsync(Z_traj, h->d_rZ, (pairs + B) * P.nz * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_rstatus, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_riters, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  CUDA_TRY(h, cudaStreamSynchronize(cs));
-  return DOJO_OK;
+    int rc = launch_grad(h, opts, n, dtraj + p0 * P.nz, dU ? dU + p0 * P.nu : nullptr, nullptr, h->d_rsol + p0 * P.nres, st + p0, h->d_Fz[k],
+                         h->d_Fu[k], nullptr, 0, nullptr, nullptr, s);
+    if (rc == DOJO_OK) leave_call(h, s);
+    return rc;
+  });
+  rc = c.finish(rc);
+  if (rc == DOJO_OK) CUDA_TRY(h, cudaStreamSynchronize(h->copy_stream));
+  return rc;
 }
 
 // The same in minimal coordinates (get_minimal_gradients! at every step): minimal_to_maximal of X0, the recording rollout, then per
@@ -1717,72 +1669,48 @@ extern "C" int dojo_rollout_grad(DojoHandle* h, const DojoSolverOptions* opts, i
 // the device), and finally maximal_to_minimal of all T + 1 slabs.  Host or device pointers (all of the same kind).
 extern "C" int dojo_rollout_minimal_gradients(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* X0, const double* U,
                                               double* X_traj, double* Gx, double* Gu, int32_t* status, int32_t* iters) {
-  int rc = rollout_grad_setup(h, B, T, X0 && X_traj && Gx && Gu, "dojo_rollout_minimal_gradients");
+  int rc = trajectory_setup(h, B, T, X0 && X_traj && Gx && Gu, "dojo_rollout_minimal_gradients", kRollGradBuffers);
+  if (rc == DOJO_OK) rc = ensure_rec_kernel(h);
+  if (rc == DOJO_OK) rc = ensure_rollout_grad_scratch(h, (size_t)B * T);
   if (rc != DOJO_OK) return rc;
   const Plan& P = h->plan;
   const size_t pairs = (size_t)B * T, nm = 2 * (size_t)P.nu, gx = nm * nm, gu = nm * P.nu;
-  const bool dev = is_device_ptr(X0), has_u = U && P.nu > 0;
-  rc = ensure_staging(h);
-  if (rc == DOJO_OK) rc = ensure_grad_chunks(h);
+  rc = ensure_grad_chunks(h);
   if (rc == DOJO_OK) rc = grow_buffer(h, (void**)&h->d_rZ, &h->rZ_bytes, (pairs + B) * P.nz * sizeof(double));
-  if (rc == DOJO_OK && !dev && has_u) rc = grow_buffer(h, (void**)&h->d_rU, &h->rU_bytes, pairs * P.nu * sizeof(double));
-  if (rc == DOJO_OK && !dev) rc = grow_buffer(h, (void**)&h->d_rX, &h->rX_bytes, std::max<size_t>(1, (pairs + B) * nm) * sizeof(double));
-  if (rc == DOJO_OK && !dev) rc = ensure_kjout(h, (size_t)h->grad_chunk * (gx + gu));
   if (rc != DOJO_OK) return rc;
   cudaStream_t s = h->stream;
-  const double* dX0 = X0;
-  const double* dU = has_u ? U : nullptr;
-  int32_t* dst = (dev && status) ? status : h->d_rstatus;
-  int32_t* dit = (dev && iters) ? iters : h->d_riters;
-  if (!dev) {
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_X, X0, (size_t)B * nm * sizeof(double), cudaMemcpyHostToDevice, s));
-    if (has_u) { CUDA_TRY(h, cudaMemcpyAsync(h->d_rU, U, pairs * P.nu * sizeof(double), cudaMemcpyHostToDevice, s)); dU = h->d_rU; }
-    dX0 = h->d_X;
-  }
+  const double *dX0 = X0, *dU = (U && P.nu > 0) ? U : nullptr;
+  double *dXt = X_traj, *cGx = nullptr, *cGu = nullptr;  // cGx, cGu: one chunk of the minimal Jacobians (host pointers)
+  int32_t *dst = status, *dit = iters;
+  HostCall c(h, X0);
+  c.in(&dX0, B * nm); c.in(&dU, pairs * P.nu); c.out(&dXt, (pairs + B) * nm); c.out(&dst, pairs); c.out(&dit, pairs);
+  c.scratch(&cGx, h->grad_chunk * gx); c.scratch(&cGu, h->grad_chunk * gu);
+  rc = c.bind();
+  if (rc != DOJO_OK) return rc;
+  int32_t* st = dst ? dst : h->d_rstatus;  // the REC kernel always writes a status
   enter_call(h, s);
   rc = launch_kin(h, true, B, dX0, h->d_rZ, s);
-  if (rc == DOJO_OK) rc = launch_rollout(h, opts, B, T, h->d_rZ, dU, nullptr, h->d_rZ + (size_t)B * P.nz, dst, s, dit, h->d_rsol);
-  if (rc != DOJO_OK) return rc;
-  for (size_t p0 = 0; p0 < pairs; p0 += h->grad_chunk) {
+  if (rc == DOJO_OK) rc = launch_rollout(h, opts, B, T, h->d_rZ, dU, nullptr, h->d_rZ + (size_t)B * P.nz, st, s, dit, h->d_rsol);
+  for (size_t p0 = 0; p0 < pairs && rc == DOJO_OK; p0 += h->grad_chunk) {
     const int n = (int)std::min<size_t>(h->grad_chunk, pairs - p0);
-    double* oGx = dev ? Gx + p0 * gx : h->d_kjout;
-    double* oGu = dev ? Gu + p0 * gu : h->d_kjout + (size_t)n * gx;
-    rc = launch_grad(h, opts, n, h->d_rZ + p0 * P.nz, dU ? dU + p0 * P.nu : nullptr, nullptr, h->d_rsol + p0 * P.nres, dst + p0, h->d_Fz[0], h->d_Fu[0],
+    double* oGx = c.dev ? Gx + p0 * gx : cGx;
+    double* oGu = c.dev ? Gu + p0 * gu : cGu;
+    rc = launch_grad(h, opts, n, h->d_rZ + p0 * P.nz, dU ? dU + p0 * P.nu : nullptr, nullptr, h->d_rsol + p0 * P.nres, st + p0, h->d_Fz[0], h->d_Fu[0],
                      nullptr, 0, nullptr, nullptr, s);
     if (rc == DOJO_OK) rc = launch_kinjac(h, 2, n, h->d_rZ + p0 * P.nz, h->d_rZ + (p0 + B) * P.nz, h->d_Fz[0], h->d_Fu[0], oGx, oGu, s);
-    if (rc != DOJO_OK) return rc;
-    if (!dev) {
+    if (rc == DOJO_OK && !c.dev) {
       CUDA_TRY(h, cudaMemcpyAsync(Gx + p0 * gx, oGx, (size_t)n * gx * sizeof(double), cudaMemcpyDeviceToHost, s));
       if (gu) CUDA_TRY(h, cudaMemcpyAsync(Gu + p0 * gu, oGu, (size_t)n * gu * sizeof(double), cudaMemcpyDeviceToHost, s));
     }
   }
-  rc = launch_kin(h, false, (int)(pairs + B), h->d_rZ, dev ? X_traj : h->d_rX, s);
-  if (rc != DOJO_OK) return rc;
-  if (!dev) {
-    CUDA_TRY(h, cudaMemcpyAsync(X_traj, h->d_rX, (pairs + B) * nm * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_rstatus, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_riters, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  }
-  leave_call(h, s);
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  if (rc == DOJO_OK) rc = launch_kin(h, false, (int)(pairs + B), h->d_rZ, dXt, s);
+  if (rc == DOJO_OK) leave_call(h, s);
+  return c.finish(rc);
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // Reverse mode through a rollout: the recording rollout without the Jacobians (tape) and its adjoint pass (include/dojo_b200.h)
 // ------------------------------------------------------------------------------------------------------------
-// Shared by the host- and device-pointer entries of both calls: no launch before every check has passed
-static int tape_vjp_setup(DojoHandle* h, int B, int T, bool buffers, const char* who) {
-  if (!h) return DOJO_EINVAL;
-  if (B <= 0 || B > h->max_batch || T <= 0 || !buffers || (long long)B * (T + 1) > (long long)INT_MAX - 2) {
-    h->err = std::string(who) + ": bad arguments (B in 1..max_batch, T >= 1, B * (T + 1) < 2^31 - 2, the required buffers)";
-    return DOJO_EINVAL;
-  }
-  if (!h->grad_bytes) { h->err = std::string(who) + ": the gradient workspace does not fit in shared memory for this mechanism"; return DOJO_ENOMEM; }
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  return DOJO_OK;
-}
-
 // the REC launch of dojo_rollout_grad without the gradient kernel and without publishing pairs: the caller's tape is its sol_raw
 static int launch_tape(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZ_traj, double* dtape,
                        int32_t* dstatus, int32_t* diters, cudaStream_t s) {
@@ -1820,92 +1748,50 @@ static int launch_vjp(DojoHandle* h, int B, int T, const double* dZ_traj, const 
 
 extern "C" int dojo_rollout_tape_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const double* dU, double* dZ_traj,
                                        double* dtape, int32_t* dstatus, int32_t* diters, void* cuda_stream) {
-  int rc = tape_vjp_setup(h, B, T, dZ0 && dZ_traj && dtape, "dojo_rollout_tape_async");
+  int rc = trajectory_setup(h, B, T, dZ0 && dZ_traj && dtape, "dojo_rollout_tape_async", "the required buffers");
   if (rc != DOJO_OK) return rc;
   return launch_tape(h, opts, B, T, dZ0, dU, dZ_traj, dtape, dstatus, diters, (cudaStream_t)cuda_stream);
 }
 
-// one grow-only buffer for the host-pointer entries, carved into the arrays of n[] (in doubles; absent arrays take no space)
-static int vjp_staging(DojoHandle* h, const size_t* n, int k, double** d) {
-  size_t total = 0;
-  for (int i = 0; i < k; ++i) total += n[i];
-  int rc = grow_buffer(h, (void**)&h->d_vjp, &h->vjp_bytes, std::max<size_t>(total, 1) * sizeof(double));
-  if (rc != DOJO_OK) return rc;
-  size_t off = 0;
-  for (int i = 0; i < k; ++i) { d[i] = n[i] ? h->d_vjp + off : nullptr; off += n[i]; }
-  return DOJO_OK;
-}
-
 extern "C" int dojo_rollout_tape(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const double* U, double* Z_traj,
                                  double* tape, int32_t* status, int32_t* iters) {
-  int rc = tape_vjp_setup(h, B, T, Z0 && Z_traj && tape, "dojo_rollout_tape");
+  int rc = trajectory_setup(h, B, T, Z0 && Z_traj && tape, "dojo_rollout_tape", "the required buffers");
   if (rc != DOJO_OK) return rc;
-  cudaStream_t s = h->stream;
-  if (is_device_ptr(Z0)) {
-    rc = launch_tape(h, opts, B, T, Z0, U, Z_traj, tape, status, iters, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
   const Plan& P = h->plan;
   const size_t pairs = (size_t)B * T;
-  const bool has_u = U && P.nu > 0;
-  // [Z_traj | tape | U] and status / iterations in the rollout scratch of dojo_rollout_grad
-  const size_t n[3] = {(pairs + B) * P.nz, pairs * P.nres, has_u ? pairs * P.nu : 0};
-  double* d[3];
-  rc = vjp_staging(h, n, 3, d);
-  if (rc == DOJO_OK) rc = ensure_rollout_grad_scratch(h, pairs);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(d[0], Z0, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
-  if (has_u) CUDA_TRY(h, cudaMemcpyAsync(d[2], U, n[2] * sizeof(double), cudaMemcpyHostToDevice, s));
-  rc = launch_tape(h, opts, B, T, d[0], d[2], d[0], d[1], h->d_rstatus, h->d_riters, s);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(Z_traj, d[0], n[0] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaMemcpyAsync(tape, d[1], n[1] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_rstatus, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_riters, pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  const double *dZ0 = Z0, *dU = U;
+  double *dtraj = Z_traj, *dtape = tape;
+  int32_t *dst = status, *dit = iters;
+  HostCall c(h, Z0);
+  c.in(&dZ0, (size_t)B * P.nz); c.in(&dU, pairs * P.nu);
+  c.out(&dtraj, (pairs + B) * P.nz); c.out(&dtape, pairs * P.nres); c.out(&dst, pairs); c.out(&dit, pairs);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_tape(h, opts, B, T, dZ0, dU, dtraj, dtape, dst, dit, h->stream);
+  return c.finish(rc);
 }
 
 extern "C" int dojo_rollout_vjp_async(DojoHandle* h, int B, int T, const double* dZ_traj, const double* dU, const double* dtape, const double* dgZ,
                                       double* dgZ0, double* dgU, int32_t* dstatus, void* cuda_stream) {
-  int rc = tape_vjp_setup(h, B, T, dZ_traj && dtape && dgZ && dgZ0, "dojo_rollout_vjp_async");
+  int rc = trajectory_setup(h, B, T, dZ_traj && dtape && dgZ && dgZ0, "dojo_rollout_vjp_async", "the required buffers");
   if (rc != DOJO_OK) return rc;
   return launch_vjp(h, B, T, dZ_traj, dU, dtape, dgZ, dgZ0, dgU, dstatus, (cudaStream_t)cuda_stream);
 }
 
 extern "C" int dojo_rollout_vjp(DojoHandle* h, int B, int T, const double* Z_traj, const double* U, const double* tape, const double* gZ, double* gZ0,
                                 double* gU, int32_t* status) {
-  int rc = tape_vjp_setup(h, B, T, Z_traj && tape && gZ && gZ0, "dojo_rollout_vjp");
+  int rc = trajectory_setup(h, B, T, Z_traj && tape && gZ && gZ0, "dojo_rollout_vjp", "the required buffers");
   if (rc != DOJO_OK) return rc;
-  cudaStream_t s = h->stream;
-  if (is_device_ptr(Z_traj)) {
-    rc = launch_vjp(h, B, T, Z_traj, U, tape, gZ, gZ0, gU, status, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
   const Plan& P = h->plan;
   const size_t pairs = (size_t)B * T, ng = 12 * (size_t)P.Nb;
-  const bool has_u = U && P.nu > 0;
-  // [Z_traj | tape | U | gZ | gZ0 | gU | status]
-  const size_t n[7] = {(pairs + B) * P.nz, pairs * P.nres, has_u ? pairs * P.nu : 0, (pairs + B) * ng, B * ng, gU ? pairs * P.nu : 0,
-                       status ? ((size_t)B + 1) / 2 : 0};
-  double* d[7];
-  rc = vjp_staging(h, n, 7, d);
-  if (rc != DOJO_OK) return rc;
-  const double* src[4] = {Z_traj, tape, U, gZ};
-  for (int k = 0; k < 4; ++k)
-    if (n[k]) CUDA_TRY(h, cudaMemcpyAsync(d[k], src[k], n[k] * sizeof(double), cudaMemcpyHostToDevice, s));
-  int32_t* dst = (int32_t*)d[6];
-  rc = launch_vjp(h, B, T, d[0], d[2], d[1], d[3], d[4], d[5], dst, s);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(gZ0, d[4], n[4] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (gU && n[5]) CUDA_TRY(h, cudaMemcpyAsync(gU, d[5], n[5] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, dst, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  const double *dZt = Z_traj, *dU = U, *dtape = tape, *dgZ = gZ;
+  double *dgZ0 = gZ0, *dgU = gU;
+  int32_t* dst = status;
+  HostCall c(h, Z_traj);
+  c.in(&dZt, (pairs + B) * P.nz); c.in(&dtape, pairs * P.nres); c.in(&dU, pairs * P.nu); c.in(&dgZ, (pairs + B) * ng);
+  c.out(&dgZ0, B * ng); c.out(&dgU, pairs * P.nu); c.out(&dst, B);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_vjp(h, B, T, dZt, dU, dtape, dgZ, dgZ0, dgU, dst, h->stream);
+  return c.finish(rc);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1967,41 +1853,18 @@ extern "C" int dojo_rollout_feedback(DojoHandle* h, const DojoSolverOptions* opt
                                      double* Z_final, double* Z_traj, double* U_applied, int32_t* status_any) {
   int rc = feedback_setup(h, B, T, fb, xi, Z0 && Z_final, "dojo_rollout_feedback");
   if (rc != DOJO_OK) return rc;
-  cudaStream_t s = h->stream;
-  if (is_device_ptr(Z0)) {
-    rc = launch_feedback(h, opts, B, T, Z0, fb, xi, Z_final, Z_traj, U_applied, status_any, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
-  rc = ensure_staging(h);
-  if (rc != DOJO_OK) return rc;
-  // one grow-only buffer: [K | K_i | x_ref | u_ref | xi | U_applied | Z_traj], absent arrays take no space
   const Plan& P = h->plan;
   const size_t ne = (size_t)fb->steps * fb->envs, nx = 2 * (size_t)P.nu, nk = P.nu * nx * ne;
-  const size_t n[7] = {nk, fb->K_i ? nk : 0, fb->x_ref ? nx * ne : 0, fb->u_ref ? P.nu * ne : 0, xi ? nx * B : 0,
-                       U_applied ? (size_t)P.nu * B * T : 0, Z_traj ? (size_t)P.nz * B * T : 0};
-  const double* src[5] = {fb->K, fb->K_i, fb->x_ref, fb->u_ref, xi};
-  size_t off[8] = {0};
-  for (int k = 0; k < 7; ++k) off[k + 1] = off[k] + n[k];
-  rc = grow_buffer(h, (void**)&h->d_fb, &h->fb_bytes, off[7] * sizeof(double));
-  if (rc != DOJO_OK) return rc;
-  double* d[7];
-  for (int k = 0; k < 7; ++k) d[k] = n[k] ? h->d_fb + off[k] : nullptr;
-  const size_t zbytes = (size_t)B * P.nz * sizeof(double);
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_Z, Z0, zbytes, cudaMemcpyHostToDevice, s));
-  for (int k = 0; k < 5; ++k)
-    if (n[k]) CUDA_TRY(h, cudaMemcpyAsync(d[k], src[k], n[k] * sizeof(double), cudaMemcpyHostToDevice, s));
-  const DojoFeedback dfb = {fb->steps, fb->envs, d[0], d[1], d[2], d[3]};
-  rc = launch_feedback(h, opts, B, T, h->d_Z, &dfb, d[4], h->d_Zn, d[6], d[5], h->d_status, s);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(Z_final, h->d_Zn, zbytes, cudaMemcpyDeviceToHost, s));
-  if (n[4]) CUDA_TRY(h, cudaMemcpyAsync(xi, d[4], n[4] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (n[5]) CUDA_TRY(h, cudaMemcpyAsync(U_applied, d[5], n[5] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (n[6]) CUDA_TRY(h, cudaMemcpyAsync(Z_traj, d[6], n[6] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (status_any) CUDA_TRY(h, cudaMemcpyAsync(status_any, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  DojoFeedback dfb = *fb;
+  const double* dZ0 = Z0;
+  double *dxi = xi, *dZf = Z_final, *dUa = U_applied, *dtraj = Z_traj;
+  int32_t* dst = status_any;
+  HostCall c(h, Z0);
+  c.in(&dZ0, (size_t)B * P.nz); c.in(&dfb.K, nk); c.in(&dfb.K_i, nk); c.in(&dfb.x_ref, nx * ne); c.in(&dfb.u_ref, P.nu * ne); c.inout(&dxi, nx * B);
+  c.out(&dZf, (size_t)B * P.nz); c.out(&dUa, (size_t)P.nu * B * T); c.out(&dtraj, (size_t)P.nz * B * T); c.out(&dst, B);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_feedback(h, opts, B, T, dZ0, &dfb, dxi, dZf, dtraj, dUa, dst, h->stream);
+  return c.finish(rc);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2011,13 +1874,14 @@ extern "C" int dojo_rollout_feedback(DojoHandle* h, const DojoSolverOptions* opt
 static int lqr_threads(int nu) { return nu <= 4 ? 64 : nu <= 16 ? 128 : nu <= 24 ? 256 : 512; }
 
 // argument checks shared by both entries (no launch before every check has passed); fills the kernel arguments but the arrays
-static int lqr_setup(DojoHandle* h, int B, int T, const DojoQuadraticCost* c, const int32_t* active, bool buffers, LqrArgs* a, const char* who) {
+static int lqr_setup(DojoHandle* h, int B, int T, const DojoQuadraticCost* c, const int32_t* active, const double* X, const double* U, const double* Gx,
+                     const double* Gu, const double* mu, double* K, double* k, double* dV, int32_t* status, LqrArgs* a, const char* who) {
   if (!h) return DOJO_EINVAL;
   const int nu = h->plan.nu;
   int na = 0;
   if (active)
     for (int i = 0; i < nu; ++i) na += active[i] != 0;
-  if (B <= 0 || B > h->max_batch || T <= 0 || !buffers || !c || !c->Q || !c->R || !c->Q_final || (c->steps != 1 && c->steps != T) ||
+  if (B <= 0 || B > h->max_batch || T <= 0 || !X || !Gx || !Gu || !K || !k || !c || !c->Q || !c->R || !c->Q_final || (c->steps != 1 && c->steps != T) ||
       (c->envs != 1 && c->envs != B) || nu == 0 || (active && na == 0)) {
     h->err = std::string(who) + ": bad arguments (B in 1..max_batch, T >= 1, cost / Q / R / Q_final / X_traj / Gx / Gu / K / k required, "
              "steps in {1, T}, envs in {1, B}, the mechanism must have inputs, `active` must have a nonzero entry)";
@@ -2039,6 +1903,8 @@ static int lqr_setup(DojoHandle* h, int B, int T, const DojoQuadraticCost* c, co
   a->nu = nu; a->B = B; a->T = T; a->steps = c->steps; a->envs = c->envs;
   for (int i = 0; i < nu; ++i)
     if (!active || active[i]) a->act[a->na++] = i;
+  a->Q = c->Q; a->R = c->R; a->xg = c->x_goal; a->ug = c->u_goal; a->Qf = c->Q_final; a->xgf = c->x_goal_final;
+  a->X = X; a->U = U; a->Gx = Gx; a->Gu = Gu; a->mu = mu; a->K = K; a->k = k; a->dV = dV; a->status = status;
   return DOJO_OK;
 }
 
@@ -2056,10 +1922,8 @@ extern "C" int dojo_lqr_backward_async(DojoHandle* h, int B, int T, const DojoQu
                                        const double* dU, const double* dGx, const double* dGu, const double* dmu, double* dK, double* dk, double* ddV,
                                        int32_t* dstatus, void* cuda_stream) {
   LqrArgs a;
-  int rc = lqr_setup(h, B, T, cost, active, dX_traj && dGx && dGu && dK && dk, &a, "dojo_lqr_backward_async");
+  int rc = lqr_setup(h, B, T, cost, active, dX_traj, dU, dGx, dGu, dmu, dK, dk, ddV, dstatus, &a, "dojo_lqr_backward_async");
   if (rc != DOJO_OK) return rc;
-  a.Q = cost->Q; a.R = cost->R; a.xg = cost->x_goal; a.ug = cost->u_goal; a.Qf = cost->Q_final; a.xgf = cost->x_goal_final;
-  a.X = dX_traj; a.U = dU; a.Gx = dGx; a.Gu = dGu; a.mu = dmu; a.K = dK; a.k = dk; a.dV = ddV; a.status = dstatus;
   return launch_lqr(h, a, (cudaStream_t)cuda_stream);
 }
 
@@ -2067,40 +1931,16 @@ extern "C" int dojo_lqr_backward(DojoHandle* h, int B, int T, const DojoQuadrati
                                  const double* U, const double* Gx, const double* Gu, const double* mu, double* K, double* k, double* dV,
                                  int32_t* status) {
   LqrArgs a;
-  int rc = lqr_setup(h, B, T, cost, active, X_traj && Gx && Gu && K && k, &a, "dojo_lqr_backward");
+  int rc = lqr_setup(h, B, T, cost, active, X_traj, U, Gx, Gu, mu, K, k, dV, status, &a, "dojo_lqr_backward");
   if (rc != DOJO_OK) return rc;
-  cudaStream_t s = h->stream;
-  if (is_device_ptr(X_traj)) {
-    rc = dojo_lqr_backward_async(h, B, T, cost, active, X_traj, U, Gx, Gu, mu, K, k, dV, status, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
-  // one grow-only buffer: [Q | R | x_goal | u_goal | Q_final | x_goal_final | X_traj | U | Gx | Gu | mu | K | k | dV | status],
-  // absent arrays take no space
   const size_t nu = a.nu, nx = 2 * nu, ne = (size_t)cost->steps * cost->envs, pairs = (size_t)B * T;
-  const size_t n[15] = {nx * nx * ne, nu * nu * ne, cost->x_goal ? nx * ne : 0, cost->u_goal ? nu * ne : 0, nx * nx * cost->envs,
-                        cost->x_goal_final ? nx * cost->envs : 0, nx * (pairs + B), U ? nu * pairs : 0, nx * nx * pairs, nx * nu * pairs,
-                        mu ? (size_t)B : 0, nu * nx * pairs, nu * pairs, dV ? 2 * (size_t)B : 0, status ? ((size_t)B + 1) / 2 : 0};
-  const double* src[11] = {cost->Q, cost->R, cost->x_goal, cost->u_goal, cost->Q_final, cost->x_goal_final, X_traj, U, Gx, Gu, mu};
-  size_t off[16] = {0};
-  for (int i = 0; i < 15; ++i) off[i + 1] = off[i] + n[i];
-  rc = grow_buffer(h, (void**)&h->d_lqr, &h->lqr_bytes, off[15] * sizeof(double));
-  if (rc != DOJO_OK) return rc;
-  double* d[15];
-  for (int i = 0; i < 15; ++i) d[i] = n[i] ? h->d_lqr + off[i] : nullptr;
-  for (int i = 0; i < 11; ++i)
-    if (n[i]) CUDA_TRY(h, cudaMemcpyAsync(d[i], src[i], n[i] * sizeof(double), cudaMemcpyHostToDevice, s));
-  a.Q = d[0]; a.R = d[1]; a.xg = d[2]; a.ug = d[3]; a.Qf = d[4]; a.xgf = d[5];
-  a.X = d[6]; a.U = d[7]; a.Gx = d[8]; a.Gu = d[9]; a.mu = d[10]; a.K = d[11]; a.k = d[12]; a.dV = d[13]; a.status = (int32_t*)d[14];
-  rc = launch_lqr(h, a, s);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(K, d[11], n[11] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaMemcpyAsync(k, d[12], n[12] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (dV) CUDA_TRY(h, cudaMemcpyAsync(dV, d[13], n[13] * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, d[14], (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  HostCall c(h, X_traj);
+  c.in(&a.Q, nx * nx * ne); c.in(&a.R, nu * nu * ne); c.in(&a.xg, nx * ne); c.in(&a.ug, nu * ne); c.in(&a.Qf, nx * nx * cost->envs);
+  c.in(&a.xgf, nx * cost->envs); c.in(&a.X, nx * (pairs + B)); c.in(&a.U, nu * pairs); c.in(&a.Gx, nx * nx * pairs); c.in(&a.Gu, nx * nu * pairs);
+  c.in(&a.mu, B); c.out(&a.K, nu * nx * pairs); c.out(&a.k, nu * pairs); c.out(&a.dV, 2 * (size_t)B); c.out(&a.status, B);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_lqr(h, a, h->stream);
+  return c.finish(rc);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2174,28 +2014,15 @@ extern "C" int dojo_env_step(DojoHandle* h, const DojoSolverOptions* opts, const
                              double* reward, int32_t* done, int32_t* status, int32_t* iters) {
   if (!h || B <= 0 || B > h->max_batch || !S || !Sn || !env_spec_ok(h, spec)) { if (h) h->err = "dojo_env_step: bad arguments"; return DOJO_EINVAL; }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = h->stream;
-  if (is_device_ptr(S)) {
-    int rc = dojo_env_step_async(h, opts, spec, B, S, A, Sn, reward, done, status, iters, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
-  int rc = ensure_staging(h);
-  if (rc == DOJO_OK) rc = ensure_env_staging(h);
-  if (rc != DOJO_OK) return rc;
   const size_t ns = dojo_env_num_state(h, spec), na = dojo_env_num_action(h, spec);
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_envS, S, (size_t)B * ns * sizeof(double), cudaMemcpyHostToDevice, s));
-  if (A && na > 0) CUDA_TRY(h, cudaMemcpyAsync(h->d_envA, A, (size_t)B * na * sizeof(double), cudaMemcpyHostToDevice, s));
-  rc = dojo_env_step_async(h, opts, spec, B, h->d_envS, (A && na > 0) ? h->d_envA : nullptr, h->d_envSn, h->d_envR, h->d_envDone, h->d_status, h->d_iters, s);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(Sn, h->d_envSn, (size_t)B * ns * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (reward) CUDA_TRY(h, cudaMemcpyAsync(reward, h->d_envR, (size_t)B * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (done) CUDA_TRY(h, cudaMemcpyAsync(done, h->d_envDone, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_status, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_iters, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  const double *dS = S, *dA = A;
+  double *dSn = Sn, *dR = reward;
+  int32_t *dd = done, *dst = status, *dit = iters;
+  HostCall c(h, S);
+  c.in(&dS, B * ns); c.in(&dA, B * na); c.out(&dSn, B * ns); c.out(&dR, B); c.out(&dd, B); c.out(&dst, B); c.out(&dit, B);
+  int rc = c.bind();
+  if (rc == DOJO_OK) rc = dojo_env_step_async(h, opts, spec, B, dS, dA, dSn, dR, dd, dst, dit, h->stream);
+  return c.finish(rc);
 }
 
 extern "C" int dojo_env_reset(DojoHandle* h, const DojoEnvSpec* spec, int B, const double* s0, const int32_t* mask, double* S) {
@@ -2271,29 +2098,16 @@ extern "C" int dojo_step_record(DojoHandle* h, const DojoSolverOptions* opts, in
                                 double* diag, int32_t* status, int32_t* iters) {
   if (!h || B <= 0 || B > h->max_batch || !Z || !Zn || !storage || !diag) { if (h) h->err = "dojo_step_record: bad arguments"; return DOJO_EINVAL; }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = h->stream;
   const Plan& P = h->plan;
-  if (is_device_ptr(Z)) {
-    int rc = dojo_step_record_async(h, opts, B, Z, U, Zn, storage, diag, status, iters, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
-  int rc = ensure_staging(h);
-  if (rc == DOJO_OK) rc = ensure_record_staging(h);
-  if (rc != DOJO_OK) return rc;
-  const bool hasU = U && P.nu > 0;
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_Z, Z, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
-  if (hasU) CUDA_TRY(h, cudaMemcpyAsync(h->d_U, U, (size_t)B * P.nu * sizeof(double), cudaMemcpyHostToDevice, s));
-  rc = dojo_step_record_async(h, opts, B, h->d_Z, hasU ? h->d_U : nullptr, h->d_Zn, h->d_recS, h->d_recD, h->d_status, h->d_iters, s);
-  if (rc != DOJO_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(Zn, h->d_Zn, (size_t)B * P.nz * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaMemcpyAsync(storage, h->d_recS, (size_t)B * 12 * P.Nb * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaMemcpyAsync(diag, h->d_recD, (size_t)B * 8 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_status, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_iters, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  const double *dZ = Z, *dU = U;
+  double *dZn = Zn, *dS = storage, *dD = diag;
+  int32_t *dst = status, *dit = iters;
+  HostCall c(h, Z);
+  c.in(&dZ, (size_t)B * P.nz); c.in(&dU, (size_t)B * P.nu);
+  c.out(&dZn, (size_t)B * P.nz); c.out(&dS, (size_t)B * 12 * P.Nb); c.out(&dD, (size_t)B * 8); c.out(&dst, B); c.out(&dit, B);
+  int rc = c.bind();
+  if (rc == DOJO_OK) rc = dojo_step_record_async(h, opts, B, dZ, dU, dZn, dS, dD, dst, dit, h->stream);
+  return c.finish(rc);
 }
 
 extern "C" int dojo_simulate_record(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const double* U, double* Z_final,
@@ -2305,23 +2119,22 @@ extern "C" int dojo_simulate_record(DojoHandle* h, const DojoSolverOptions* opts
   if (rc != DOJO_OK) return rc;
   cudaStream_t s = h->stream;
   const Plan& P = h->plan;
-  const bool dev = is_device_ptr(Z0);
+  const double* dU = (U && P.nu > 0) ? U : nullptr;
+  HostCall c(h, Z0);
+  c.in(&dU, (size_t)P.nu * B * T);
+  rc = c.bind();
+  if (rc != DOJO_OK) return rc;
+  const bool dev = c.dev;
   const cudaMemcpyKind in = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, out = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   const size_t nzb = (size_t)B * P.nz * sizeof(double), nsb = (size_t)B * 12 * P.Nb * sizeof(double), ndb = (size_t)B * 8 * sizeof(double);
-  const bool hasU = U && P.nu > 0;
   CUDA_TRY(h, cudaMemcpyAsync(h->d_recZ[0], Z0, nzb, in, s));
   CUDA_TRY(h, cudaMemsetAsync(h->d_recAny, 0, (size_t)B * sizeof(int32_t), s));
   int cur = 0;
   for (int k = 0; k < T; ++k, cur ^= 1) {
-    const double* dU = nullptr;
-    if (hasU) {
-      if (dev) dU = U + (size_t)k * B * P.nu;
-      else { CUDA_TRY(h, cudaMemcpyAsync(h->d_U, U + (size_t)k * B * P.nu, (size_t)B * P.nu * sizeof(double), cudaMemcpyHostToDevice, s)); dU = h->d_U; }
-    }
     // with device pointers the per-step outputs are written in place
     double* dS = (dev && storage) ? storage + (size_t)k * B * 12 * P.Nb : h->d_recS;
     double* dD = (dev && diag) ? diag + (size_t)k * B * 8 : h->d_recD;
-    rc = dojo_step_record_async(h, opts, B, h->d_recZ[cur], dU, h->d_recZ[cur ^ 1], dS, dD, h->d_status, nullptr, s);
+    rc = dojo_step_record_async(h, opts, B, h->d_recZ[cur], dU ? dU + (size_t)k * B * P.nu : nullptr, h->d_recZ[cur ^ 1], dS, dD, h->d_status, nullptr, s);
     if (rc != DOJO_OK) return rc;
     dojo_status_max_kernel<<<(B + 255) / 256, 256, 0, s>>>(B, h->d_status, h->d_recAny);
     CUDA_TRY(h, cudaGetLastError());
@@ -2332,8 +2145,7 @@ extern "C" int dojo_simulate_record(DojoHandle* h, const DojoSolverOptions* opts
   }
   CUDA_TRY(h, cudaMemcpyAsync(Z_final, h->d_recZ[cur], nzb, out, s));
   if (status_any) CUDA_TRY(h, cudaMemcpyAsync(status_any, h->d_recAny, (size_t)B * sizeof(int32_t), out, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  return c.finish();
 }
 
 extern "C" int dojo_env_rollout(DojoHandle* h, const DojoSolverOptions* opts, const DojoEnvSpec* spec, int B, int T, const double* S0, const double* A,
@@ -2344,28 +2156,27 @@ extern "C" int dojo_env_rollout(DojoHandle* h, const DojoSolverOptions* opts, co
   if (rc == DOJO_OK) rc = ensure_env_staging(h);
   if (rc != DOJO_OK) return rc;
   cudaStream_t s = h->stream;
-  const bool dev = is_device_ptr(S0);
-  const cudaMemcpyKind in = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, out = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   const size_t ns = dojo_env_num_state(h, spec), na = dojo_env_num_action(h, spec);
+  const double* dA = (A && na > 0) ? A : nullptr;
+  HostCall c(h, S0);
+  c.in(&dA, na * B * T);
+  rc = c.bind();
+  if (rc != DOJO_OK) return rc;
+  const cudaMemcpyKind in = c.dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, out = c.dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   double* buf[2] = {h->d_envS, h->d_envSn};
   CUDA_TRY(h, cudaMemcpyAsync(buf[0], S0, (size_t)B * ns * sizeof(double), in, s));
   CUDA_TRY(h, cudaMemsetAsync(h->d_envR, 0, (size_t)B * sizeof(double), s));        // return accumulator
   CUDA_TRY(h, cudaMemsetAsync(h->d_envDone, 0, (size_t)B * sizeof(int32_t), s));    // failure flags
   int cur = 0;
   for (int k = 0; k < T; ++k, cur ^= 1) {
-    const double* dA = nullptr;
-    if (A && na > 0) {
-      if (dev) dA = A + (size_t)k * B * na;
-      else { CUDA_TRY(h, cudaMemcpyAsync(h->d_envA, A + (size_t)k * B * na, (size_t)B * na * sizeof(double), cudaMemcpyHostToDevice, s)); dA = h->d_envA; }
-    }
-    rc = env_step_impl(h, opts, spec, B, buf[cur], dA, buf[cur ^ 1], nullptr, nullptr, h->d_status, nullptr, h->d_envR, h->d_envDone, s);
+    rc = env_step_impl(h, opts, spec, B, buf[cur], dA ? dA + (size_t)k * B * na : nullptr, buf[cur ^ 1], nullptr, nullptr, h->d_status, nullptr, h->d_envR,
+                       h->d_envDone, s);
     if (rc != DOJO_OK) return rc;
   }
   CUDA_TRY(h, cudaMemcpyAsync(S_final, buf[cur], (size_t)B * ns * sizeof(double), out, s));
   if (ret) CUDA_TRY(h, cudaMemcpyAsync(ret, h->d_envR, (size_t)B * sizeof(double), out, s));
   if (failed) CUDA_TRY(h, cudaMemcpyAsync(failed, h->d_envDone, (size_t)B * sizeof(int32_t), out, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  return c.finish();
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2410,17 +2221,15 @@ extern "C" int dojo_env_policy_rollout(DojoHandle* h, const DojoSolverOptions* o
   if (rc == DOJO_OK) rc = ensure_env_staging(h);
   if (rc != DOJO_OK) return rc;
   cudaStream_t s = h->stream;
-  const bool dev = is_device_ptr(S0);
-  const cudaMemcpyKind in = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, out = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   const size_t ns = dojo_env_num_state(h, spec), na = dojo_env_num_action(h, spec);
   if (na == 0) { h->err = "dojo_env_policy_rollout: the environment has no actions"; return DOJO_EINVAL; }
   if (!h->d_envNorm) CUDA_TRY(h, cudaMalloc((void**)&h->d_envNorm, 2 * (2 * (size_t)h->plan.nu + h->plan.Ni) * sizeof(double)));
   const double* dTheta = Theta;
-  if (!dev) {
-    if (!h->d_envTheta) CUDA_TRY(h, cudaMalloc((void**)&h->d_envTheta, (size_t)h->max_batch * h->plan.nu * (2 * (size_t)h->plan.nu + h->plan.Ni) * sizeof(double)));
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_envTheta, Theta, (size_t)B * ns * na * sizeof(double), cudaMemcpyHostToDevice, s));
-    dTheta = h->d_envTheta;
-  }
+  HostCall c(h, S0);
+  c.in(&dTheta, B * ns * na);
+  rc = c.bind();
+  if (rc != DOJO_OK) return rc;
+  const cudaMemcpyKind in = c.dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, out = c.dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   if (mean) {
     CUDA_TRY(h, cudaMemcpyAsync(h->d_envNorm, mean, ns * sizeof(double), cudaMemcpyHostToDevice, s));
     CUDA_TRY(h, cudaMemcpyAsync(h->d_envNorm + ns, stdev, ns * sizeof(double), cudaMemcpyHostToDevice, s));
@@ -2444,8 +2253,7 @@ extern "C" int dojo_env_policy_rollout(DojoHandle* h, const DojoSolverOptions* o
   CUDA_TRY(h, cudaMemcpyAsync(S_final, buf[cur], (size_t)B * ns * sizeof(double), out, s));
   if (ret) CUDA_TRY(h, cudaMemcpyAsync(ret, h->d_envR, (size_t)B * sizeof(double), out, s));
   if (failed) CUDA_TRY(h, cudaMemcpyAsync(failed, h->d_envDone, (size_t)B * sizeof(int32_t), out, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  return c.finish();
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2459,35 +2267,27 @@ extern "C" int dojo_step_grad_contact(DojoHandle* h, const DojoSolverOptions* op
   CUDA_TRY(h, cudaSetDevice(h->device));
   const Plan& P = h->plan;
   cudaStream_t s = h->stream;
-  if (is_device_ptr(Z)) {
-    int rc = dojo_step_grad_contact_async(h, opts, B, Z, U, nullptr, Zn, Fz, Fu, Fc, status, iters, 0, s);
-    if (rc != DOJO_OK) return rc;
-    CUDA_TRY(h, cudaStreamSynchronize(s));
-    return DOJO_OK;
-  }
-  int rc = ensure_staging(h);
-  if (rc != DOJO_OK) return rc;
+  HostCall c(h, Z);
+  if (c.dev) return c.finish(dojo_step_grad_contact_async(h, opts, B, Z, U, nullptr, Zn, Fz, Fu, Fc, status, iters, 0, s));
   const size_t ng = 12 * (size_t)P.Nb, fz = ng * ng, fu = ng * P.nu, fc = ng * 5 * P.Ni;
   // chunks of environments whose three Jacobians fit 192 MB of device staging
   const int chunk = (int)std::max<size_t>(1, std::min<size_t>(B, (size_t(192) << 20) / ((fz + fu + fc) * sizeof(double))));
-  rc = ensure_kjout(h, (size_t)chunk * (fz + fu + fc));
+  const double *dZ = Z, *dU = U;
+  double *dZn = Zn, *dFz = nullptr;
+  int32_t *dst = status, *dit = iters;
+  c.in(&dZ, (size_t)B * P.nz); c.in(&dU, (size_t)B * P.nu); c.out(&dZn, (size_t)B * P.nz); c.out(&dst, B); c.out(&dit, B);
+  c.scratch(&dFz, (size_t)chunk * (fz + fu + fc));
+  int rc = c.bind();
   if (rc != DOJO_OK) return rc;
-  double *dFz = h->d_kjout, *dFu = dFz + (size_t)chunk * fz, *dFc = dFu + (size_t)chunk * fu;
-  const bool hasU = U && P.nu > 0;
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_Z, Z, (size_t)B * P.nz * sizeof(double), cudaMemcpyHostToDevice, s));
-  if (hasU) CUDA_TRY(h, cudaMemcpyAsync(h->d_U, U, (size_t)B * P.nu * sizeof(double), cudaMemcpyHostToDevice, s));
-  for (int e0 = 0; e0 < B; e0 += chunk) {
+  double *dFu = dFz + (size_t)chunk * fz, *dFc = dFu + (size_t)chunk * fu;
+  for (int e0 = 0; e0 < B && rc == DOJO_OK; e0 += chunk) {
     const int nb = std::min(chunk, B - e0);
-    rc = dojo_step_grad_contact_async(h, opts, nb, h->d_Z + (size_t)e0 * P.nz, hasU ? h->d_U + (size_t)e0 * P.nu : nullptr, nullptr,
-                                      h->d_Zn + (size_t)e0 * P.nz, dFz, dFu, dFc, h->d_status + e0, h->d_iters + e0, 0, s);
-    if (rc != DOJO_OK) return rc;
+    rc = dojo_step_grad_contact_async(h, opts, nb, dZ + (size_t)e0 * P.nz, dU ? dU + (size_t)e0 * P.nu : nullptr, nullptr, dZn + (size_t)e0 * P.nz, dFz, dFu,
+                                      dFc, dst ? dst + e0 : nullptr, dit ? dit + e0 : nullptr, 0, s);
+    if (rc != DOJO_OK) break;
     CUDA_TRY(h, cudaMemcpyAsync(Fz + (size_t)e0 * fz, dFz, (size_t)nb * fz * sizeof(double), cudaMemcpyDeviceToHost, s));
     if (fu) CUDA_TRY(h, cudaMemcpyAsync(Fu + (size_t)e0 * fu, dFu, (size_t)nb * fu * sizeof(double), cudaMemcpyDeviceToHost, s));
     if (fc) CUDA_TRY(h, cudaMemcpyAsync(Fc + (size_t)e0 * fc, dFc, (size_t)nb * fc * sizeof(double), cudaMemcpyDeviceToHost, s));
   }
-  CUDA_TRY(h, cudaMemcpyAsync(Zn, h->d_Zn, (size_t)B * P.nz * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_status, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (iters) CUDA_TRY(h, cudaMemcpyAsync(iters, h->d_iters, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(h, cudaStreamSynchronize(s));
-  return DOJO_OK;
+  return c.finish(rc);
 }

@@ -42,10 +42,13 @@
  * Gradients use the 12-per-body attitude-reduced packing [x(3) v(3) phi(3) w(3)]
  * (src/gradients/state.jl:102-123), column-major [12Nb x 12Nb] and [12Nb x nu] per environment.
  *
- * Buffers passed to dojo_step / dojo_step_grad / dojo_rollout may be HOST or DEVICE pointers
- * (detected with cudaPointerGetAttributes); host buffers are staged through pinned memory and
- * copied inside the call.  The *_async variants take device pointers only and a cudaStream_t
- * (passed as void*), do not synchronise, and are what a resident-data caller uses.
+ * Buffers passed to the synchronous entries (dojo_step, dojo_step_grad, dojo_rollout, ...) may be
+ * HOST or DEVICE pointers, all of one call of the same kind (detected with cudaPointerGetAttributes
+ * on the first array); host buffers are copied inside the call.  dojo_step / dojo_step_trace stage
+ * pageable buffers through the handle's pinned memory; every other entry copies directly from / to
+ * the caller's buffers, through one grow-only device staging arena per handle.  The *_async variants
+ * take device pointers only and a cudaStream_t (passed as void*), do not synchronise, and are what a
+ * resident-data caller uses.
  *
  * Threading / streams: a handle is not thread-safe (the reference's Mechanism is single-threaded and mutable as well) and
  * has ONE call in flight at a time: the work-queue counter, completion lists, staging and scratch buffers belong to the
