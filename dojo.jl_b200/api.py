@@ -275,6 +275,58 @@ def get_trajectory_vjp(mechanism: Mechanism, z0, U, gZ, opts=None, device: int =
     return traj, gZ0, gU, status
 
 
+def _sum_like(g, given, tail):
+    """a per-environment law gradient g [steps, B, *tail] summed to the shape of the law array it belongs to (feedback_arrays' shapes:
+    tail, [B, *tail], [T, 1, *tail] or [T, B, *tail]); sums in a fixed order over the steps, then the environments"""
+    given = np.asarray(given)
+    if given.ndim == len(tail) + 2:
+        s_g, e_g = given.shape[0], given.shape[1]
+    elif given.ndim == len(tail) + 1:
+        s_g, e_g = 1, given.shape[0]
+    else:
+        s_g, e_g = 1, 1
+    if s_g == 1 and g.shape[0] > 1:
+        g = g.sum(axis=0, keepdims=True)
+    if e_g == 1 and g.shape[1] > 1:
+        g = g.sum(axis=1, keepdims=True)
+    return g.reshape(given.shape)
+
+
+def get_feedback_vjp(mechanism: Mechanism, z0, control: "LinearFeedback", steps: int, gZ=None, gX=None, gU=None, opts=None, device: int = 0):
+    """The vector-Jacobian product of simulate(mechanism, steps, z0, control=LinearFeedback(...)) with respect to the law and the start:
+    the closed loop recorded on the device (dojo_rollout_feedback_tape), then one adjoint pass (dojo_rollout_feedback_vjp).  Cotangents,
+    each optional: gZ [steps+1, B, 12Nb] on the states (packing [x, v, phi, w] per body), gX [steps+1, B, 2nu] on the law's minimal
+    states x_t, gU [steps, B, nu] on the applied inputs (for a single environment without the B axis).  Returns a dict: the gradients
+    K, K_i, x_ref, u_ref shaped like the law's arrays (summed over the environments and steps an array is shared by; None for an absent
+    array), xi (the gradient with respect to the law's starting integral state, None without K_i), gZ0 [B, 12Nb], and the record:
+    Z_traj [steps+1, B, 13Nb], X_traj [steps+1, B, 2nu], U [steps, B, nu], status [steps, B] (3 at every step of an environment whose
+    backward pass met a non-finite factorisation; its gradients are then NaN).  control.xi is not updated."""
+    z0 = np.asarray(z0, dtype=float)
+    single = z0.ndim == 1
+    Z0 = np.atleast_2d(z0)
+    B = Z0.shape[0]
+    lift = (lambda a: None if a is None else np.asarray(a, dtype=float)[:, None]) if single else (lambda a: a)  # noqa: E731
+    s = _stepper(mechanism, B, device)
+    fb = control
+    law = dict(K=fb.K, x_ref=fb.x_ref, u_ref=fb.u_ref, K_i=fb.K_i)
+    rec = s.rollout_feedback_tape(Z0, steps, xi=fb.xi, opts=opts, **law)
+    g = s.rollout_feedback_vjp(rec, gZ=lift(gZ), gX=lift(gX), gU=lift(gU), **law)
+    nu = s.nu
+    tails = dict(K=(nu, 2 * nu), K_i=(nu, 2 * nu), x_ref=(2 * nu,), u_ref=(nu,))
+    out = {k: None if law[k] is None else _sum_like(g[k], law[k], tails[k]) for k in tails}
+    xi = g["gxi0"]
+    if xi is not None and (fb.xi is None or np.ndim(fb.xi) == 1):
+        xi = xi.sum(axis=0) if not single else xi[0]
+    status = np.where(g["status"][None, :] != 0, g["status"][None, :], rec["status"])
+    res = dict(out, xi=xi, gZ0=g["gZ0"], Z_traj=rec["Z_traj"], X_traj=rec["X_traj"], U=rec["U"], status=status)
+    if single:
+        for k in ("gZ0",):
+            res[k] = res[k][0]
+        for k in ("Z_traj", "X_traj", "U", "status"):
+            res[k] = res[k][:, 0]
+    return res
+
+
 def get_minimal_trajectory_gradients(mechanism: Mechanism, x0, U, opts=None, device: int = 0):
     """get_trajectory_gradients in minimal coordinates (get_minimal_gradients! at every step): x0 [2nu], U [T, nu] -> (X_traj [T+1, 2nu],
     Gx [T, 2nu, 2nu], Gu [T, 2nu, nu], status [T]).  The rollout runs in maximal coordinates from minimal_to_maximal(x0); X_traj is its

@@ -1,4 +1,5 @@
-"""PyTorch autograd through a fused rollout: rollout(mechanism, Z0, U) is differentiable with respect to Z0 and U.
+"""PyTorch autograd through a fused rollout: rollout(mechanism, Z0, U) is differentiable with respect to Z0 and U, and
+rollout_feedback(mechanism, Z0, K, ...) through a closed loop with respect to Z0 and the linear law's tensors.
 
     from dojo_jl_b200.autograd import rollout
     Z_traj, status = rollout(mech, Z0, U)           # CUDA fp64: Z0 [B, 13Nb], U [T, B, nu] -> Z_traj [T+1, B, 13Nb], status [T, B]
@@ -126,3 +127,119 @@ def rollout(mechanism: Mechanism, Z0, U, opts=None):
         raise ValueError(f"rollout: Z0 [B, {mechanism.nz}] and U [T, B, {mechanism.nu}] expected, got {tuple(Z0.shape)} and {tuple(U.shape)}")
     s = _stepper(mechanism, Z0.shape[0], Z0.device.index if Z0.device.index is not None else torch.cuda.current_device())
     return _Rollout.apply(Z0, U, s, opts)
+
+
+def _feedback_function():
+    import torch
+
+    class RolloutFeedback(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, Z0, K, u_ref, x_ref, K_i, xi0, stepper, opts, T, steps, envs):
+            B, dev, nu = Z0.shape[0], Z0.device, stepper.nu
+            nx = 2 * nu
+
+            def lay(a, tail, mat):  # [steps, envs, *tail] contiguous; matrices column-major per entry
+                if a is None:
+                    return None
+                a = a.detach()
+                a = a.reshape((1, 1) + tail) if a.dim() == len(tail) else (a.unsqueeze(0) if a.dim() == len(tail) + 1 else a)
+                a = a.expand((steps, envs) + tail)
+                return (a.transpose(-1, -2) if mat else a).contiguous()
+
+            Kc, Kic = lay(K, (nu, nx), True), lay(K_i, (nu, nx), True)
+            xrc, urc = lay(x_ref, (nx,), False), lay(u_ref, (nu,), False)
+            f64 = dict(dtype=torch.float64, device=dev)
+            xi = None if K_i is None else (torch.zeros((B, nx), **f64) if xi0 is None else xi0.detach().expand(B, nx).contiguous().clone())
+            Z_traj, X_traj = torch.empty((T + 1, B, stepper.nz), **f64), torch.empty((T + 1, B, nx), **f64)
+            Xi = None if K_i is None else torch.empty((T, B, nx), **f64)
+            Ua, tape = torch.empty((T, B, nu), **f64), torch.empty((T, B, stepper.nres), **f64)
+            p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            stepper.rollout_feedback_tape_device(Z0.detach().contiguous().data_ptr(), Z_traj.data_ptr(), X_traj.data_ptr(), Ua.data_ptr(),
+                                                 tape.data_ptr(), B, T, Kc.data_ptr(), steps=steps, envs=envs, dK_i=p(Kic), dx_ref=p(xrc),
+                                                 du_ref=p(urc), dxi=p(xi), dXi_traj=p(Xi), opts=opts, stream=stream)
+            ctx.save_for_backward(Z_traj, X_traj, Ua, tape, Kc, Kic, xrc, urc, Xi)
+            ctx.stepper, ctx.steps, ctx.envs = stepper, steps, envs
+            ctx.shapes = [None if a is None else a.shape for a in (K, u_ref, x_ref, K_i, xi0)]
+            return Z_traj, X_traj, Ua
+
+        @staticmethod
+        def backward(ctx, gZ_traj, gX_traj, gUa):
+            Z_traj, X_traj, Ua, tape, Kc, Kic, xrc, urc, Xi = ctx.saved_tensors
+            s, steps = ctx.stepper, ctx.steps
+            T, B = tape.shape[0], tape.shape[1]
+            nu, nx, dev = s.nu, 2 * s.nu, Z_traj.device
+            f64 = dict(dtype=torch.float64, device=dev)
+            gZ = None if gZ_traj is None else to_attitude(Z_traj, gZ_traj.to(torch.float64)).contiguous()
+            gX = None if gX_traj is None else gX_traj.to(torch.float64).contiguous()
+            gU = None if gUa is None else gUa.to(torch.float64).contiguous()
+            shp = dict(zip(("K", "u_ref", "x_ref", "K_i", "xi0"), ctx.shapes))
+            gK = torch.empty((steps, B, nx, nu), **f64) if ctx.needs_input_grad[1] else None
+            gur = torch.empty((steps, B, nu), **f64) if ctx.needs_input_grad[2] else None
+            gxr = torch.empty((steps, B, nx), **f64) if ctx.needs_input_grad[3] else None
+            gKi = torch.empty((steps, B, nx, nu), **f64) if ctx.needs_input_grad[4] else None
+            gZ0 = torch.empty((B, s.ngrad), **f64)
+            gxi0 = None if Kic is None else torch.empty((B, nx), **f64)
+            p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            s.rollout_feedback_vjp_device(Z_traj.data_ptr(), X_traj.data_ptr(), Ua.data_ptr(), tape.data_ptr(), gZ0.data_ptr(), B, T, Kc.data_ptr(),
+                                          steps=steps, envs=ctx.envs, dK_i=p(Kic), dx_ref=p(xrc), du_ref=p(urc), dXi_traj=p(Xi), dgZ=p(gZ),
+                                          dgX=p(gX), dgU=p(gU), dgK=p(gK), dgK_i=p(gKi), dgx_ref=p(gxr), dgu_ref=p(gur), dgxi0=p(gxi0),
+                                          stream=stream)
+
+            def fit(g, name, mat):  # per-environment [steps, B, ...] -> the input's shape, broadcast dimensions summed
+                if g is None or shp[name] is None:
+                    return None
+                g = g.transpose(-1, -2) if mat else g
+                n = len(shp[name]) - (2 if mat else 1)  # leading (step / environment) axes of the input
+                if n == 0:
+                    return g.sum(dim=(0, 1))
+                if n == 1:
+                    return g.sum(dim=0)
+                return g.sum(dim=1, keepdim=True) if shp[name][1] == 1 else g
+
+            gxi = None
+            if gxi0 is not None and ctx.needs_input_grad[5]:
+                gxi = gxi0.sum(dim=0) if len(shp["xi0"]) == 1 else gxi0
+            return (from_attitude(Z_traj[0], gZ0), fit(gK, "K", True), fit(gur, "u_ref", False), fit(gxr, "x_ref", False), fit(gKi, "K_i", True),
+                    gxi, None, None, None, None, None)
+
+    return RolloutFeedback
+
+
+_RolloutFeedback = None
+
+
+def rollout_feedback(mechanism: Mechanism, Z0, K, u_ref=None, x_ref=None, K_i=None, xi0=None, opts=None, T=None):
+    """T closed-loop steps of B environments under u_t = u_ref - K (x_t - x_ref) - K_i xi_t (dojo_rollout_feedback's law),
+    differentiable with respect to Z0 [B, 13Nb], K, u_ref, x_ref, K_i and xi0 (CUDA float64 tensors on one device).  Each law tensor
+    is [*tail], [B, *tail] or [T, 1 or B, *tail] (tail: [nu, 2nu] for K / K_i, [nu] for u_ref, [2nu] for x_ref); xi0 [2nu] or [B, 2nu]
+    (zero when None).  T is taken from a tensor with a step axis, else it must be given.  Returns (Z_traj [T+1, B, 13Nb], X_traj
+    [T+1, B, 2nu] (the law's x_t; slab T = maximal_to_minimal(z_T)), U_applied [T, B, nu]).  The backward pass maps the quaternion
+    cotangents of Z_traj as rollout() does and returns each input's gradient summed over its broadcast dimensions."""
+    import torch
+    global _RolloutFeedback
+    if _RolloutFeedback is None:
+        _RolloutFeedback = _feedback_function()
+    nu = mechanism.nu
+    tails = {"K": (nu, 2 * nu), "u_ref": (nu,), "x_ref": (2 * nu,), "K_i": (nu, 2 * nu)}
+    given = {k: a for k, a in zip(tails, (K, u_ref, x_ref, K_i)) if a is not None}
+    for a in list(given.values()) + [Z0] + ([xi0] if xi0 is not None else []):
+        if not torch.is_tensor(a) or a.dtype != torch.float64 or not a.is_cuda or a.device != Z0.device:
+            raise ValueError("rollout_feedback: Z0 and the law's tensors must be float64 CUDA tensors on one device")
+    B = Z0.shape[0]
+    steps, envs = 1, 1
+    for k, a in given.items():
+        n = a.dim() - len(tails[k])
+        if n not in (0, 1, 2) or tuple(a.shape[n:]) != tails[k] or (n == 1 and a.shape[0] != B) or (n == 2 and a.shape[1] not in (1, B)):
+            raise ValueError(f"rollout_feedback: {k} of shape {tuple(a.shape)}")
+        if n == 2:
+            if T is not None and a.shape[0] != T:
+                raise ValueError(f"rollout_feedback: {k} has {a.shape[0]} steps, T = {T}")
+            T, steps = a.shape[0], a.shape[0]
+        if (n == 1) or (n == 2 and a.shape[1] == B):
+            envs = B
+    if T is None:
+        raise ValueError("rollout_feedback: T is required when no law tensor has a step axis")
+    s = _stepper(mechanism, B, Z0.device.index if Z0.device.index is not None else torch.cuda.current_device())
+    return _RolloutFeedback.apply(Z0, K, u_ref, x_ref, K_i, xi0, s, opts, int(T), steps, envs)

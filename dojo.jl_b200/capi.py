@@ -62,6 +62,12 @@ class DojoFeedback(C.Structure):
     _fields_ = [("steps", C.c_int32), ("envs", C.c_int32), ("K", c_double_p), ("K_i", c_double_p), ("x_ref", c_double_p), ("u_ref", c_double_p)]
 
 
+class DojoFeedbackGrad(C.Structure):
+    """Law gradients of dojo_rollout_feedback_vjp (include/dojo_b200.h: DojoFeedbackGrad), each nullable and always per environment:
+    [.. x B x steps] with the DojoFeedback's steps; K / K_i column-major [nu x 2nu] per entry."""
+    _fields_ = [("K", c_double_p), ("K_i", c_double_p), ("x_ref", c_double_p), ("u_ref", c_double_p)]
+
+
 class DojoQuadraticCost(C.Structure):
     """Quadratic tracking cost of dojo_lqr_backward (include/dojo_b200.h: DojoQuadraticCost).  Q, R, x_goal, u_goal hold steps (1 or T) x
     envs (1 or B) entries, Q_final and x_goal_final envs entries; matrices column-major per entry."""

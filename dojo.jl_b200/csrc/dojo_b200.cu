@@ -66,6 +66,20 @@ static const void* step_vjp_kernel_fn(bool any_contact, bool plan_smem) {
   if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<true, true, false, false, false, false, true>;
   return (const void*)dojo_step_kernel<true, false, false, false, false, false, true>;
 }
+// the closed-loop tape (REC + FB, dojo_rollout_feedback_tape) and its adjoint (VJP + FB, dojo_rollout_feedback_vjp), placed as the FB and
+// the VJP kernel
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_fbtape_kernel();
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_fbvjp_kernel();
+static const void* step_fbtape_kernel_fn(bool any_contact, bool plan_smem) {
+  if (any_contact) return dojo_cm_step_fbtape_kernel();
+  if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<false, true, false, false, true, true>;
+  return (const void*)dojo_step_kernel<false, false, false, false, true, true>;
+}
+static const void* step_fbvjp_kernel_fn(bool any_contact, bool plan_smem) {
+  if (any_contact) return dojo_cm_step_fbvjp_kernel();
+  if (plan_smem && !getenv("DOJO_B200_GENERIC_PLAN")) return (const void*)dojo_step_kernel<true, true, false, false, false, true, true>;
+  return (const void*)dojo_step_kernel<true, false, false, false, false, true, true>;
+}
 
 // Order of the work queue.  A per-step launch ends when its slowest environment ends: an environment that stalls (ten line-search
 // trials per iteration up to max_iter, ~6 x the median time) and is dequeued late finishes alone.  Which environments stall is not
@@ -224,6 +238,11 @@ struct DojoHandle {
   double* d_fbX = nullptr;                         // FB scratch: x_t [2nu x max_batch], then u_t [nu x max_batch] (no U_applied)
   bool lqr_ready = false;                          // dojo_lqr_backward_kernel has the device's shared-memory maximum
   const void* k_vjp = nullptr;                     // adjoint kernel (VJP), set up by the first dojo_rollout_vjp call
+  const void* k_fb_tape = nullptr;                 // closed-loop tape (REC + FB), set up by the first dojo_rollout_feedback_tape call
+  const void* k_fb_vjp = nullptr;                  // closed-loop adjoint (VJP + FB), set up by the first dojo_rollout_feedback_vjp call
+  int envs_per_sm_fb_tape = 1;
+  double* d_fbvws = nullptr;                       // closed-loop adjoint scratch of the device-pointer calls (grow-only)
+  size_t fbvws_bytes = 0;
   std::string err;
 };
 // Whether the forward kernel specialised for small mechanisms (dojo_step_kernel.cuh, SMALL) computes this handle's step exactly: the
@@ -816,6 +835,7 @@ extern "C" int dojo_destroy(DojoHandle* h) {
   cudaFree(h->d_stage);
   cudaFree(h->d_rsol); cudaFree(h->d_rdone); cudaFree(h->d_rstatus); cudaFree(h->d_riters); cudaFree(h->d_rZ);
   cudaFree(h->d_fbX);
+  cudaFree(h->d_fbvws);
   delete h;
   return DOJO_OK;
 }
@@ -1811,8 +1831,8 @@ static int ensure_fb_kernel(DojoHandle* h) {
   return DOJO_OK;
 }
 
-// argument checks shared by both entries: no launch before every check has passed
-static int feedback_setup(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* xi, bool buffers, const char* who) {
+// argument checks of the closed-loop entries (dojo_rollout_feedback and its tape / adjoint): no launch before every check has passed
+static int feedback_check(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* xi, bool buffers, const char* who) {
   if (!h) return DOJO_EINVAL;
   if (B <= 0 || B > h->max_batch || T <= 0 || !buffers || !fb || !fb->K || (fb->steps != 1 && fb->steps != T) || (fb->envs != 1 && fb->envs != B) ||
       (fb->K_i && !xi) || h->plan.nu == 0) {
@@ -1821,7 +1841,11 @@ static int feedback_setup(DojoHandle* h, int B, int T, const DojoFeedback* fb, c
     return DOJO_EINVAL;
   }
   CUDA_TRY(h, cudaSetDevice(h->device));
-  return ensure_fb_kernel(h);
+  return DOJO_OK;
+}
+static int feedback_setup(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* xi, bool buffers, const char* who) {
+  int rc = feedback_check(h, B, T, fb, xi, buffers, who);
+  return rc == DOJO_OK ? ensure_fb_kernel(h) : rc;
 }
 
 // fb's arrays are device pointers here
@@ -1864,6 +1888,158 @@ extern "C" int dojo_rollout_feedback(DojoHandle* h, const DojoSolverOptions* opt
   c.out(&dZf, (size_t)B * P.nz); c.out(&dUa, (size_t)P.nu * B * T); c.out(&dtraj, (size_t)P.nz * B * T); c.out(&dst, B);
   rc = c.bind();
   if (rc == DOJO_OK) rc = launch_feedback(h, opts, B, T, dZ0, &dfb, dxi, dZf, dtraj, dUa, dst, h->stream);
+  return c.finish(rc);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Reverse mode through the closed loop: the feedback tape and its adjoint (include/dojo_b200.h)
+// ------------------------------------------------------------------------------------------------------------
+// argument checks of both entries (no launch before every check has passed): the feedback rollout's rules and the tape's buffers
+static int feedback_tape_setup(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* xi, const double* Xi_traj, bool buffers,
+                               const char* who) {
+  if (!h) return DOJO_EINVAL;
+  if (!fb || (!fb->K_i != !Xi_traj)) {
+    h->err = std::string(who) + ": bad arguments (feedback required; Xi_traj is required if and only if K_i is given)";
+    return DOJO_EINVAL;
+  }
+  int rc = trajectory_setup(h, B, T, buffers, who, "Z_traj / X_traj / U_applied / tape required");
+  if (rc == DOJO_OK) rc = feedback_check(h, B, T, fb, xi, true, who);
+  return rc;
+}
+
+static int launch_feedback_tape(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const DojoFeedback* fb, double* dxi,
+                                double* dZ_traj, double* dX_traj, double* dXi_traj, double* dUa, double* dtape, int32_t* dstatus, int32_t* diters,
+                                cudaStream_t s) {
+  if (!h->k_fb_tape) {
+    const void* k = step_fbtape_kernel_fn(h->any_contact, h->plan_smem_mask == 0xff);
+    int occ = 1;
+    CUDA_TRY(h, max_shared_memory(k, h->device));
+    CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, 32 * h->nw * h->slots, h->smem_fwd));
+    h->envs_per_sm_fb_tape = std::max(1, occ);
+    h->k_fb_tape = k;
+  }
+  if (!dstatus) {  // the REC kernel always writes a status
+    int rc = ensure_rollout_grad_scratch(h, (size_t)B * T);
+    if (rc != DOJO_OK) return rc;
+  }
+  StepArgs a = step_args(h, opts, B, false);
+  a.Z = dZ_traj; a.traj = dZ_traj + (size_t)B * h->plan.nz; a.T = T;
+  a.sol_raw = dtape; a.status = dstatus ? dstatus : h->d_rstatus; a.iters = diters;
+  a.fb_K = fb->K; a.fb_Ki = fb->K_i; a.fb_xref = fb->x_ref; a.fb_uref = fb->u_ref; a.fb_steps = fb->steps; a.fb_envs = fb->envs;
+  a.fb_xi = dxi; a.fb_u = dUa; a.fb_u_T = 1; a.fb_xtraj = dX_traj; a.fb_xitraj = dXi_traj;
+  enter_call(h, s);
+  if (dZ0 != dZ_traj) CUDA_TRY(h, cudaMemcpyAsync(dZ_traj, dZ0, (size_t)B * h->plan.nz * sizeof(double), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
+  const int grid = std::min((B + h->slots - 1) / h->slots, h->sm_count * h->envs_per_sm_fb_tape);
+  { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(h->k_fb_tape, dim3(grid), dim3(32 * h->nw * h->slots), kargs, h->smem_fwd, s)); }
+  CUDA_TRY(h, cudaGetLastError());
+  h->launches += 1;
+  leave_call(h, s);
+  return DOJO_OK;
+}
+
+extern "C" int dojo_rollout_feedback_tape_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const DojoFeedback* fb,
+                                                double* dxi, double* dZ_traj, double* dX_traj, double* dXi_traj, double* dU_applied, double* dtape,
+                                                int32_t* dstatus, int32_t* diters, void* cuda_stream) {
+  int rc = feedback_tape_setup(h, B, T, fb, dxi, dXi_traj, dZ0 && dZ_traj && dX_traj && dU_applied && dtape, "dojo_rollout_feedback_tape_async");
+  if (rc != DOJO_OK) return rc;
+  return launch_feedback_tape(h, opts, B, T, dZ0, fb, dxi, dZ_traj, dX_traj, dXi_traj, dU_applied, dtape, dstatus, diters, (cudaStream_t)cuda_stream);
+}
+
+extern "C" int dojo_rollout_feedback_tape(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const DojoFeedback* fb, double* xi,
+                                          double* Z_traj, double* X_traj, double* Xi_traj, double* U_applied, double* tape, int32_t* status,
+                                          int32_t* iters) {
+  int rc = feedback_tape_setup(h, B, T, fb, xi, Xi_traj, Z0 && Z_traj && X_traj && U_applied && tape, "dojo_rollout_feedback_tape");
+  if (rc != DOJO_OK) return rc;
+  const Plan& P = h->plan;
+  const size_t pairs = (size_t)B * T, ne = (size_t)fb->steps * fb->envs, nx = 2 * (size_t)P.nu, nk = P.nu * nx * ne;
+  DojoFeedback dfb = *fb;
+  const double* dZ0 = Z0;
+  double *dxi = xi, *dtraj = Z_traj, *dX = X_traj, *dXi = Xi_traj, *dUa = U_applied, *dtape = tape;
+  int32_t *dst = status, *dit = iters;
+  HostCall c(h, Z0);
+  c.in(&dZ0, (size_t)B * P.nz); c.in(&dfb.K, nk); c.in(&dfb.K_i, nk); c.in(&dfb.x_ref, nx * ne); c.in(&dfb.u_ref, P.nu * ne); c.inout(&dxi, nx * B);
+  c.out(&dtraj, (pairs + B) * P.nz); c.out(&dX, (pairs + B) * nx); c.out(&dXi, pairs * nx); c.out(&dUa, pairs * P.nu); c.out(&dtape, pairs * P.nres);
+  c.out(&dst, pairs); c.out(&dit, pairs);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_feedback_tape(h, opts, B, T, dZ0, &dfb, dxi, dtraj, dX, dXi, dUa, dtape, dst, dit, h->stream);
+  return c.finish(rc);
+}
+
+// the adjoint's checks: the tape's, the cotangents' and the gradient workspace (which also holds the per-joint contributions of M' w)
+static int feedback_vjp_setup(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* Xi_traj, const double* gxi0, bool buffers,
+                              const char* who) {
+  if (h && fb && fb->K_i && !gxi0) { h->err = std::string(who) + ": bad arguments (gxi0 is required with K_i)"; return DOJO_EINVAL; }
+  int rc = feedback_tape_setup(h, B, T, fb, fb && fb->K_i ? gxi0 : nullptr, Xi_traj, buffers, who);
+  if (rc != DOJO_OK) return rc;
+  const Plan& P = h->plan;
+  if ((size_t)24 * P.Ne > (size_t)P.n_red * P.ch) { h->err = std::string(who) + ": the gradient workspace does not fit for this mechanism"; return DOJO_ENOMEM; }
+  return DOJO_OK;
+}
+
+static int launch_feedback_vjp(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* dZ_traj, const double* dX_traj, const double* dXi_traj,
+                               const double* dUa, const double* dtape, const double* dgZ, const double* dgX, const double* dgUa, const DojoFeedbackGrad* out,
+                               double* dgZ0, double* dgxi0, int32_t* dstatus, double* dws, cudaStream_t s) {
+  if (!h->k_fb_vjp) {
+    const void* k = step_fbvjp_kernel_fn(h->any_contact, h->plan_smem_mask_grad == 0xff);
+    CUDA_TRY(h, max_shared_memory(k, h->device));
+    h->k_fb_vjp = k;
+  }
+  StepArgs a = step_args(h, nullptr, B, true);
+  a.Z = dZ_traj; a.U = dUa; a.sol_raw = const_cast<double*>(dtape); a.status = dstatus; a.T = T;
+  a.vjp_gZ = dgZ; a.vjp_lam = dgZ0;
+  a.fb_K = fb->K; a.fb_Ki = fb->K_i; a.fb_xref = fb->x_ref; a.fb_uref = fb->u_ref; a.fb_steps = fb->steps; a.fb_envs = fb->envs; a.fb_xi = dgxi0;
+  a.fb_xtraj = const_cast<double*>(dX_traj); a.fb_xitraj = const_cast<double*>(dXi_traj); a.fbv_gX = dgX; a.fbv_gUa = dgUa;
+  if (out) { a.fbv_gK = out->K; a.fbv_gKi = fb->K_i ? out->K_i : nullptr; a.fbv_gxref = out->x_ref; a.fbv_guref = out->u_ref; }
+  a.fbv_ws = dws;
+  enter_call(h, s);
+  CUDA_TRY(h, cudaMemsetAsync(h->d_counter, 0, sizeof(int), s));
+  const int grid = std::min((B + h->slots_grad - 1) / h->slots_grad, h->sm_count * h->envs_per_sm_grad);
+  { void* kargs[1] = {(void*)&a}; CUDA_TRY(h, cudaLaunchKernel(h->k_fb_vjp, dim3(grid), dim3(32 * h->nw * h->slots_grad), kargs, h->smem_grad, s)); }
+  CUDA_TRY(h, cudaGetLastError());
+  h->launches += 1;
+  leave_call(h, s);
+  return DOJO_OK;
+}
+static size_t feedback_vjp_ws(const Plan& P, int B) { return ((size_t)4 * P.nu + 12 * (size_t)P.Nb) * B; }
+
+extern "C" int dojo_rollout_feedback_vjp_async(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* dZ_traj, const double* dX_traj,
+                                               const double* dXi_traj, const double* dU_applied, const double* dtape, const double* dgZ,
+                                               const double* dgX, const double* dgUa, const DojoFeedbackGrad* out, double* dgZ0, double* dgxi0,
+                                               int32_t* dstatus, void* cuda_stream) {
+  int rc = feedback_vjp_setup(h, B, T, fb, dXi_traj, dgxi0, dZ_traj && dX_traj && dU_applied && dtape && dgZ0, "dojo_rollout_feedback_vjp_async");
+  if (rc == DOJO_OK) rc = grow_buffer(h, (void**)&h->d_fbvws, &h->fbvws_bytes, feedback_vjp_ws(h->plan, B) * sizeof(double));
+  if (rc != DOJO_OK) return rc;
+  return launch_feedback_vjp(h, B, T, fb, dZ_traj, dX_traj, dXi_traj, dU_applied, dtape, dgZ, dgX, dgUa, out, dgZ0, dgxi0, dstatus, h->d_fbvws,
+                             (cudaStream_t)cuda_stream);
+}
+
+extern "C" int dojo_rollout_feedback_vjp(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* Z_traj, const double* X_traj,
+                                         const double* Xi_traj, const double* U_applied, const double* tape, const double* gZ, const double* gX,
+                                         const double* gUa, const DojoFeedbackGrad* out, double* gZ0, double* gxi0, int32_t* status) {
+  int rc = feedback_vjp_setup(h, B, T, fb, Xi_traj, gxi0, Z_traj && X_traj && U_applied && tape && gZ0, "dojo_rollout_feedback_vjp");
+  if (rc != DOJO_OK) return rc;
+  const Plan& P = h->plan;
+  const size_t pairs = (size_t)B * T, ne = (size_t)fb->steps * fb->envs, nx = 2 * (size_t)P.nu, nk = P.nu * nx, ng = 12 * (size_t)P.Nb;
+  const size_t no = (size_t)fb->steps * B;  // entries of each gradient output
+  DojoFeedback dfb = *fb;
+  DojoFeedbackGrad dout = {};
+  if (out) dout = *out;
+  if (!fb->K_i) dout.K_i = nullptr;
+  const double *dZt = Z_traj, *dX = X_traj, *dXi = Xi_traj, *dUa = U_applied, *dtape = tape, *dgZ = gZ, *dgX = gX, *dgUa = gUa;
+  double *dgZ0 = gZ0, *dgxi0 = fb->K_i ? gxi0 : nullptr, *dws = nullptr;
+  int32_t* dst = status;
+  HostCall c(h, Z_traj);
+  c.in(&dfb.K, nk * ne); c.in(&dfb.K_i, nk * ne); c.in(&dfb.x_ref, nx * ne); c.in(&dfb.u_ref, P.nu * ne);
+  c.in(&dZt, (pairs + B) * P.nz); c.in(&dX, (pairs + B) * nx); c.in(&dXi, pairs * nx); c.in(&dUa, pairs * P.nu); c.in(&dtape, pairs * P.nres);
+  c.in(&dgZ, (pairs + B) * ng); c.in(&dgX, (pairs + B) * nx); c.in(&dgUa, pairs * P.nu);
+  c.out(&dout.K, nk * no); c.out(&dout.K_i, nk * no); c.out(&dout.x_ref, nx * no); c.out(&dout.u_ref, P.nu * no);
+  c.out(&dgZ0, B * ng); c.out(&dgxi0, B * nx); c.out(&dst, B);
+  c.scratch(&dws, feedback_vjp_ws(P, B));
+  rc = c.bind();
+  if (rc == DOJO_OK && c.dev) rc = grow_buffer(h, (void**)&h->d_fbvws, &h->fbvws_bytes, feedback_vjp_ws(P, B) * sizeof(double));
+  if (rc == DOJO_OK) rc = launch_feedback_vjp(h, B, T, &dfb, dZt, dX, dXi, dUa, dtape, dgZ, dgX, dgUa, &dout, dgZ0, dgxi0, dst, c.dev ? h->d_fbvws : dws,
+                                              h->stream);
   return c.finish(rc);
 }
 

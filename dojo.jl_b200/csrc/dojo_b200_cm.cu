@@ -36,3 +36,10 @@ extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_fb_ker
 extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_vjp_kernel() {
   return (const void*)dj_cm::dojo_step_kernel<true, false, false, false, false, false, true>;
 }
+// the closed-loop tape and its adjoint of this compilation (dojo_rollout_feedback_tape / dojo_rollout_feedback_vjp)
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_fbtape_kernel() {
+  return (const void*)dj_cm::dojo_step_kernel<false, false, false, false, true, true>;
+}
+extern "C" __attribute__((visibility("hidden"))) const void* dojo_cm_step_fbvjp_kernel() {
+  return (const void*)dj_cm::dojo_step_kernel<true, false, false, false, false, true, true>;
+}

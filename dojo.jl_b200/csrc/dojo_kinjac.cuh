@@ -138,6 +138,81 @@ DJ_DEV void max_to_min_block(const JointDev& jd, const BodyState& A, const BodyS
     for (int r = 0; r < 2 * nuj; ++r) for (int c = 0; c < 12; ++c) blk[(size_t)r * 24 + c] = 0.0;
 }
 
+// The same block contracted with a cotangent: out[24] = blk' w for w = the joint's 2 nu_j entries of a minimal-state cotangent, without
+// forming blk (the adjoint of the closed loop, dojo_step_kernel.cuh: add_max_to_min_vjp).  The partials are max_to_min_block's, each
+// applied to the same mask rows; a world parent's 12 entries are zero.
+DJ_DEV void max_to_min_vjp_joint(const JointDev& jd, const BodyState& A, const BodyState& Bc, double h, const double* w, double* out) {
+  const int nt = jd.nfree_t, nr = jd.nfree_r, nuj = nt + nr;
+  for (int i = 0; i < 24; ++i) out[i] = 0.0;
+  // out[c0 .. c0 + 2] += w_r (D' a)
+  auto acc = [&](int c0, double wr, V3 r) { out[c0] += wr * r.x; out[c0 + 1] += wr * r.y; out[c0 + 2] += wr * r.z; };
+  const double ih = 1.0 / h;
+  const V3 pa = v3(jd.pa[0], jd.pa[1], jd.pa[2]), pb = v3(jd.pb[0], jd.pb[1], jd.pb[2]);
+  const Quat ma = qmap(-A.w, h), mb = qmap(-Bc.w, h);
+  const Quat qa1 = qmul(A.q, ma), qb1 = qmul(Bc.q, mb);
+  const M33 RmaT = transpose(rotmat(ma)), RmbT = transpose(rotmat(mb));
+  const M33 Ea = attitude_velocity_jacobian(-A.w, h), Eb = attitude_velocity_jacobian(-Bc.w, h);
+  if (nt > 0) {
+    const V3 xa1 = A.x - h * A.v, xb1 = Bc.x - h * Bc.v;
+    const M33 Ra = rotmat(A.q), Rb = rotmat(Bc.q), Ra1 = rotmat(qa1), Rb1 = rotmat(qb1);
+    const V3 e = tra_displacement(jd, A.x, A.q, Bc.x, Bc.q), e1 = tra_displacement(jd, xa1, qa1, xb1, qb1);
+    const M33 RaT = transpose(Ra), Ra1T = transpose(Ra1);
+    const M33 c_pa = 2.0 * skew(e + pa);
+    const M33 c_pb = (-2.0) * (RaT * Rb * skew(pb));
+    const M33 c1_pa0 = 2.0 * skew(e1 + pa);
+    const M33 c1_pb0 = (-2.0) * (Ra1T * Rb1 * skew(pb));
+    const M33 v_xa = ih * (Ra1T - RaT), v_va = (-1.0) * Ra1T, v_pa = ih * (c_pa - c1_pa0 * RmaT), v_wa = ih * (c1_pa0 * Ea);
+    const M33 v_xb = ih * (RaT - Ra1T), v_vb = Ra1T, v_pb = ih * (c_pb - c1_pb0 * RmbT), v_wb = ih * (c1_pb0 * Eb);
+    for (int i = 0; i < nt; ++i) {
+      const V3 a = mask_row(jd.At, i);
+      const double wc = w[i], wv = w[nuj + i];
+      acc(0, wc, -1.0 * tmul(RaT, a));  acc(6, wc, tmul(c_pa, a));  acc(12, wc, tmul(RaT, a));  acc(18, wc, tmul(c_pb, a));
+      acc(0, wv, tmul(v_xa, a));  acc(3, wv, tmul(v_va, a));  acc(6, wv, tmul(v_pa, a));  acc(9, wv, tmul(v_wa, a));
+      acc(12, wv, tmul(v_xb, a)); acc(15, wv, tmul(v_vb, a)); acc(18, wv, tmul(v_pb, a)); acc(21, wv, tmul(v_wb, a));
+    }
+  }
+  if (nr > 0) {
+    const Quat qoff = Quat{jd.qoff[0], jd.qoff[1], jd.qoff[2], jd.qoff[3]};
+    const Quat qoffi = qinv(qoff);
+    const M33 RoffT = transpose(rotmat(qoff));
+    const Quat q = qmul(qmul(qoffi, qinv(A.q)), Bc.q);
+    const Quat q1 = qmul(qmul(qoffi, qinv(qa1)), qb1);
+    const Quat p = qmul(qinv(q1), q);
+    const M34 Dq = drotation_vector_dq(q), Dp = drotation_vector_dq(p);
+    const M33 c_pb = D_LVt(Dq, q);
+    const M33 c_pa = (-1.0) * (D_RVt(Dq, q) * RoffT);
+    const M33 DRp = D_RVt(Dp, p);
+    const M33 K = DRp * transpose(rotmat(q1)) * RoffT;
+    const M33 v_pb = ih * (D_LVt(Dp, p) - DRp * RmbT);
+    const M33 v_wb = ih * (DRp * Eb);
+    const M33 v_pa = ih * (K * (RmaT - m33ident()));
+    const M33 v_wa = (-ih) * (K * Ea);
+    for (int i = 0; i < nr; ++i) {
+      const V3 a = mask_row(jd.Ar, i);
+      const double wc = w[nt + i], wv = w[nuj + nt + i];
+      acc(6, wc, tmul(c_pa, a));  acc(18, wc, tmul(c_pb, a));
+      acc(6, wv, tmul(v_pa, a));  acc(9, wv, tmul(v_wa, a));  acc(18, wv, tmul(v_pb, a));  acc(21, wv, tmul(v_wb, a));
+    }
+  }
+  if (jd.parent < 0)  // the origin is not a variable
+    for (int c = 0; c < 12; ++c) out[c] = 0.0;
+}
+
+// body b's 12 entries of M' w from the per-joint contributions contrib [Ne][24] of max_to_min_vjp_joint: the joints b is the parent or
+// the child of, in joint order
+DJ_DEV void max_to_min_vjp_fold(const JointDev* joints, int Ne, int b, const double* contrib, double* g) {
+  for (int k = 0; k < 12; ++k) g[k] = 0.0;
+  for (int j = 0; j < Ne; ++j) {
+    const JointDev& jd = joints[j];
+    if (jd.nfree_t + jd.nfree_r == 0) continue;
+    const double* s = contrib + (size_t)24 * j;
+    if (jd.parent == b)
+      for (int k = 0; k < 12; ++k) g[k] += s[k];
+    if (jd.child == b)
+      for (int k = 0; k < 12; ++k) g[k] += s[12 + k];
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ N: one body
 // Partials of set_minimal_coordinates_velocities! (joints/minimal.jl:148-203) for the child of joint jd:
 //   Pm [12][12] row-major: d(xb, vb, phi_b, wb) / d(Dx, Dtheta, Dv, Dw)  (2 nu_j columns used)   (:314-400)
@@ -326,7 +401,7 @@ DJ_DEV void kinjac_env(const KinJacArgs& a, int e, double* ws, int tid, int nthr
   }
 }
 
-#if defined(__CUDACC__) || defined(DJ_HOSTEMU)
+#if defined(DJ_HOSTEMU) || (defined(__CUDACC__) && !defined(DJ_ANY_CONTACT))  // dojo_b200_cm.cu includes the routines above only
 // persistent grid: CTA b takes environments b, b + gridDim.x, ...; workspace slice b
 __global__ void __launch_bounds__(128) dojo_kinjac_kernel(const KinJacArgs a) {
   double* ws = a.ws + (size_t)blockIdx.x * kinjac_ws_doubles(a.Nb, a.nu);

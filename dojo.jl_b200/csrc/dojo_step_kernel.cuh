@@ -10,6 +10,7 @@
 #include "../../include/dojo_b200.h"
 #include "dojo_grad.cuh"
 #include "dojo_kin.cuh"
+#include "dojo_kinjac.cuh"
 
 namespace dj {
 
@@ -73,7 +74,34 @@ struct StepArgs {
   const double* vjp_gZ;  // [12Nb x B x (T + 1)]
   double* vjp_lam;       // [12Nb x B]: lambda_t of the step the owning slot is at; gZ0 = lambda_0 on return
   double* vjp_gU;        // nullable [nu x B x T]
+  // closed-loop tape and adjoint (REC + FB kernels: dojo_rollout_feedback_tape; VJP + FB kernels: dojo_rollout_feedback_vjp).  The law's
+  // arrays are fb_K .. fb_envs; the VJP + FB kernel reads the applied inputs from a.U and keeps nu, the adjoint of the integral, in fb_xi
+  // [2nu x B] (required iff fb_Ki).  Gradient outputs hold fb_steps x B entries, entry (t, e) at (fb_steps > 1 ? t : 0) * B + e; with
+  // fb_steps = 1 the slot sums them over t.  After vjp_gU, so that no other member moves.
+  double* fb_xtraj;       // [2nu x B x (T + 1)]: x_t of every step and x_T = m(z_T) (written by REC + FB, read by VJP + FB)
+  double* fb_xitraj;      // [2nu x B x T]: xi_t (required iff fb_Ki)
+  const double* fbv_gX;   // nullable [2nu x B x (T + 1)]: cotangents of x_t
+  const double* fbv_gUa;  // nullable [nu x B x T]: cotangents of the applied inputs
+  double* fbv_gK;         // nullable [nu x 2nu x B x fb_steps], as K
+  double* fbv_gKi;        // nullable, as K_i
+  double* fbv_gxref;      // nullable [2nu x B x fb_steps]
+  double* fbv_guref;      // nullable [nu x B x fb_steps]
+  double* fbv_ws;         // [fbv_ws_doubles x B] scratch
 };
+
+// per-environment scratch of the VJP + FB kernel: Fu' lambda [nu] | a [nu] | d_bar + gX [2nu] | zero cotangent [12 Nb]
+DJ_DEV size_t fbv_ws_doubles(const Plan& P) { return (size_t)4 * P.nu + 12 * (size_t)P.Nb; }
+
+// the KKT blocks of recorded pair p, assembled at its final iterate (the tape), as the gradient pass has them before gradients()
+DJ_DEV void vjp_restore(Ctx& c, const StepArgs& a, size_t p, const double* u) {
+  const Plan& P = *c.P;
+  prologue(c, a.Z + p * P.nz, u, nullptr, true);
+  for (int k = c.tid; k < P.nres; k += c.nthreads) c.A[P.sol_off + k] = a.sol_raw[p * P.nres + k];
+  slot_sync(c);
+  double rv, bv;
+  c.mu = 0.0;
+  evaluate<true>(c, 0.0, P.rhs_off, rv, bv);
+}
 
 // adjoint pass of the VJP kernel for environment e (dojo_rollout_vjp): lambda_T = gZ[T]; for t = T-1 .. 0 the gradient pass's
 // prologue, tape and assembly at pair t * B + e, then vjp_step (dojo_grad.cuh): gU[t] = Fu_t' lambda_{t+1}, lambda_t = Fz_t' lambda_{t+1}
@@ -90,12 +118,7 @@ DJ_DEV int rollout_vjp(Ctx& c, const StepArgs& a, int e) {
   for (int t = a.T - 1; t >= 0 && ok; --t) {
     const size_t p = (size_t)t * a.B + e;
     const double* u = a.U ? a.U + p * P.nu : nullptr;
-    prologue(c, a.Z + p * P.nz, u, nullptr, true);
-    for (int k = c.tid; k < P.nres; k += c.nthreads) c.A[P.sol_off + k] = a.sol_raw[p * P.nres + k];
-    slot_sync(c);
-    double rv, bv;
-    c.mu = 0.0;
-    evaluate<true>(c, 0.0, P.rhs_off, rv, bv);
+    vjp_restore(c, a, p, u);
     ok = vjp_step(c, u, lam, a.vjp_gZ + p * ng, a.vjp_gU ? a.vjp_gU + p * P.nu : nullptr);
   }
   if (ok) return 0;
@@ -108,10 +131,12 @@ DJ_DEV int rollout_vjp(Ctx& c, const StepArgs& a, int e) {
 
 // feedback stage of the FB kernel for environment e before step t from state z (global memory); returns where u_t was written.
 // Lanes: one per joint for the map (max_to_min_joint reads only the joint's parent and child), one per entry of xi, one per input.
+// REC (the closed-loop tape): x_t goes to slab t of a.fb_xtraj instead of the scratch, and xi_t to slab t of a.fb_xitraj.
+template <bool REC = false>
 DJ_DEV const double* feedback(Ctx& c, const StepArgs& a, const double* z, int e, int t) {
   const Plan& P = *c.P;
   const int nu = P.nu, nx = 2 * nu;
-  double* x = a.fb_x + (size_t)e * nx;
+  double* x = REC ? a.fb_xtraj + ((size_t)t * a.B + e) * nx : a.fb_x + (size_t)e * nx;
   for (int j = c.tid; j < P.Ne; j += c.nthreads) max_to_min_joint(c.joints[j], P.h, z, x);
   __threadfence_block();
   slot_sync(c);
@@ -119,7 +144,10 @@ DJ_DEV const double* feedback(Ctx& c, const StepArgs& a, const double* z, int e,
   const double* xr = a.fb_xref ? a.fb_xref + q * nx : nullptr;
   double* xi = a.fb_Ki ? a.fb_xi + (size_t)e * nx : nullptr;
   if (xi) {  // the integral is updated before it is used (pendulum_pid.jl)
-    for (int k = c.tid; k < nx; k += c.nthreads) xi[k] += P.h * (xr ? x[k] - xr[k] : x[k]);
+    for (int k = c.tid; k < nx; k += c.nthreads) {
+      xi[k] += P.h * (xr ? x[k] - xr[k] : x[k]);
+      if (REC) a.fb_xitraj[((size_t)t * a.B + e) * nx + k] = xi[k];
+    }
     __threadfence_block();
     slot_sync(c);
   }
@@ -136,6 +164,124 @@ DJ_DEV const double* feedback(Ctx& c, const StepArgs& a, const double* z, int e,
   __threadfence_block();
   slot_sync(c);
   return u;
+}
+
+// M_t' w added to lambda (lam, 12 Nb), M_t the Jacobian of the minimal state at z: one lane per joint for its contribution to its parent
+// and child (the gradient vectors' region of the arena as per-joint scratch, which the next step's gradient pass rebuilds), then one
+// lane per body for the sum of its joints' contributions, in joint order.
+DJ_DEV void add_max_to_min_vjp(Ctx& c, const double* z, const double* w, double* lam) {
+  const Plan& P = *c.P;
+  double* s = c.A + P.gvec_off;
+  for (int j = c.tid; j < P.Ne; j += c.nthreads) {
+    const JointDev& jd = c.joints[j];
+    if (jd.nfree_t + jd.nfree_r > 0) max_to_min_vjp_joint(jd, kin_load(z, jd.parent), kin_load(z, jd.child), P.h, w + 2 * jd.u_off, s + (size_t)24 * j);
+  }
+  slot_sync(c);
+  for (int b = c.tid; b < P.Nb; b += c.nthreads) {
+    double g[12];
+    max_to_min_vjp_fold(c.joints, P.Ne, b, s, g);
+    for (int k = 0; k < 12; ++k) lam[12 * b + k] += g[k];
+  }
+  __threadfence_block();
+  slot_sync(c);
+}
+
+// adjoint pass of the VJP + FB kernel for environment e (dojo_rollout_feedback_vjp): the step adjoint of rollout_vjp() at the applied
+// inputs, then the adjoint of the law.  With a_t = Fu_t' lambda_{t+1} + gUa[t] and d_t = x_t - x_ref:
+//   nu <- nu - K_i' a_t,  d_bar = -K' a_t + h nu,  lambda_t = Fz_t' lambda_{t+1} + gZ[t] + M_t' (d_bar + gX[t]),
+//   dK = -a_t d_t',  dK_i = -a_t xi_t',  du_ref = a_t,  dx_ref = -d_bar;   lambda_T = gZ[T] + M_T' gX[T].
+// One lane per entry of a, nu, d_bar and of the gain gradients; gZ0 = lambda_0, gxi0 = nu.  Returns 0, or 3 when a factorisation was
+// not finite (every output of the environment is then NaN).
+DJ_DEV int rollout_feedback_vjp(Ctx& c, const StepArgs& a, int e) {
+  const Plan& P = *c.P;
+  const int ng = 12 * P.Nb, nu = P.nu, nx = 2 * nu, nk = nu * nx;
+  const bool tiled = a.fb_steps > 1;
+  double* lam = a.vjp_lam + (size_t)e * ng;
+  double* nv = a.fb_Ki ? a.fb_xi + (size_t)e * nx : nullptr;
+  double* gu = a.fbv_ws + (size_t)e * fbv_ws_doubles(P);
+  double* av = gu + nu;
+  double* w = av + nu;
+  double* gz0 = w + nx;  // the cotangent of z_t when the caller gives none
+  const size_t zT = (size_t)a.T * a.B + e;
+  for (int k = c.tid; k < ng; k += c.nthreads) { lam[k] = a.vjp_gZ ? a.vjp_gZ[zT * ng + k] : 0.0; gz0[k] = 0.0; }
+  if (nv)
+    for (int k = c.tid; k < nx; k += c.nthreads) nv[k] = 0.0;
+  if (!tiled) {  // sums over t
+    for (int k = c.tid; k < nk; k += c.nthreads) {
+      if (a.fbv_gK) a.fbv_gK[(size_t)e * nk + k] = 0.0;
+      if (a.fbv_gKi) a.fbv_gKi[(size_t)e * nk + k] = 0.0;
+    }
+    for (int k = c.tid; k < nx; k += c.nthreads) if (a.fbv_gxref) a.fbv_gxref[(size_t)e * nx + k] = 0.0;
+    for (int k = c.tid; k < nu; k += c.nthreads) if (a.fbv_guref) a.fbv_guref[(size_t)e * nu + k] = 0.0;
+  }
+  __threadfence_block();
+  slot_sync(c);
+  if (a.fbv_gX) add_max_to_min_vjp(c, a.Z + zT * P.nz, a.fbv_gX + zT * nx, lam);
+  bool ok = true;
+  for (int t = a.T - 1; t >= 0 && ok; --t) {
+    const size_t p = (size_t)t * a.B + e;
+    const double* u = a.U + p * nu;
+    vjp_restore(c, a, p, u);
+    ok = vjp_step(c, u, lam, a.vjp_gZ ? a.vjp_gZ + p * ng : gz0, gu);
+    if (!ok) break;
+    const size_t q = (size_t)(tiled ? t : 0) * a.fb_envs + (a.fb_envs > 1 ? e : 0);  // the law's entry
+    const size_t o = (size_t)(tiled ? t : 0) * a.B + e;                                 // the gradients' entry
+    const double* K = a.fb_K + q * nk;
+    const double* Ki = a.fb_Ki ? a.fb_Ki + q * nk : nullptr;
+    const double* xr = a.fb_xref ? a.fb_xref + q * nx : nullptr;
+    const double* x = a.fb_xtraj + p * nx;
+    const double* xi = a.fb_Ki ? a.fb_xitraj + p * nx : nullptr;
+    for (int i = c.tid; i < nu; i += c.nthreads) {
+      const double ai = a.fbv_gUa ? gu[i] + a.fbv_gUa[p * nu + i] : gu[i];
+      av[i] = ai;
+      if (a.fbv_guref) { if (tiled) a.fbv_guref[o * nu + i] = ai; else a.fbv_guref[o * nu + i] += ai; }
+    }
+    __threadfence_block();
+    slot_sync(c);
+    for (int k = c.tid; k < nx; k += c.nthreads) {
+      double s = 0.0;
+      for (int i = 0; i < nu; ++i) s += K[i + (size_t)nu * k] * av[i];
+      double db = -s;
+      if (Ki) {
+        double si = 0.0;
+        for (int i = 0; i < nu; ++i) si += Ki[i + (size_t)nu * k] * av[i];
+        nv[k] = nv[k] - si;
+        db = P.h * nv[k] - s;
+      }
+      if (a.fbv_gxref) { if (tiled) a.fbv_gxref[o * nx + k] = -db; else a.fbv_gxref[o * nx + k] -= db; }
+      w[k] = a.fbv_gX ? db + a.fbv_gX[p * nx + k] : db;
+    }
+    for (int k = c.tid; k < nk; k += c.nthreads) {
+      const int i = k % nu, j = k / nu;
+      if (a.fbv_gK) {
+        const double g = -av[i] * (xr ? x[j] - xr[j] : x[j]);
+        if (tiled) a.fbv_gK[o * nk + k] = g; else a.fbv_gK[o * nk + k] += g;
+      }
+      if (a.fbv_gKi) {
+        const double g = -av[i] * xi[j];
+        if (tiled) a.fbv_gKi[o * nk + k] = g; else a.fbv_gKi[o * nk + k] += g;
+      }
+    }
+    __threadfence_block();
+    slot_sync(c);
+    add_max_to_min_vjp(c, a.Z + p * P.nz, w, lam);
+  }
+  if (ok) return 0;
+  const double qnan = nan("");
+  for (int k = c.tid; k < ng; k += c.nthreads) lam[k] = qnan;
+  if (nv)
+    for (int k = c.tid; k < nx; k += c.nthreads) nv[k] = qnan;
+  const int ns = tiled ? a.T : 1;
+  for (int k = c.tid; k < ns * nk; k += c.nthreads) {
+    const size_t o = (size_t)(k / nk) * a.B + e;
+    if (a.fbv_gK) a.fbv_gK[o * nk + k % nk] = qnan;
+    if (a.fbv_gKi) a.fbv_gKi[o * nk + k % nk] = qnan;
+  }
+  for (int k = c.tid; k < ns * nx; k += c.nthreads)
+    if (a.fbv_gxref) a.fbv_gxref[((size_t)(k / nx) * a.B + e) * nx + k % nx] = qnan;
+  for (int k = c.tid; k < ns * nu; k += c.nthreads)
+    if (a.fbv_guref) a.fbv_guref[((size_t)(k / nu) * a.B + e) * nu + k % nu] = qnan;
+  return 3;
 }
 
 // epilogue: update_state! + get_next_state (bodies/set.jl:22-36, mechanism/get.jl:126-134).  The default output is the
@@ -185,15 +331,19 @@ __device__ __forceinline__ unsigned long long k_t0g(unsigned long long* prof) { 
 // FB (forward, untraced, generic): the closed-loop rollout of dojo_rollout_feedback.  Before the prologue of step t the slot evaluates the
 // linear feedback law on the state the step starts from (feedback() above) and the step reads u_t from a.fb_u; a.U is not read.  The step
 // itself is dojo_rollout's.  A compile-time parameter, like REC.
+// REC + FB: the closed-loop tape of dojo_rollout_feedback_tape.  The FB rollout, recorded like REC (a.fb_u holds the applied inputs
+// [nu x B x T]), which also keeps the law's x_t in a.fb_xtraj, xi_t in a.fb_xitraj and, after the last step, x_T = m(z_T).
 // VJP (gradient): the adjoint pass of dojo_rollout_vjp.  A slot takes an environment from the work queue and walks its recorded steps
 // backwards (rollout_vjp() above), one transposed solve per step instead of the gradient kernel's column solves.  Same launch
 // configuration and arena as the gradient kernel; a compile-time parameter, so that the other instantiations are the same code.
+// VJP + FB: the adjoint of the closed loop (dojo_rollout_feedback_vjp, rollout_feedback_vjp() above): VJP's step adjoint at the applied
+// inputs a.U, followed per step by the adjoint of the law.
 template <bool GRAD, bool PLAN_SMEM = false, bool TRACE = false, bool SMALL = false, bool REC = false, bool FB = false, bool VJP = false>
 __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(const StepArgs a) {
   static_assert(!SMALL || (!GRAD && PLAN_SMEM && !TRACE), "SMALL is a specialisation of the untraced forward kernel with the plan in shared memory");
   static_assert(!REC || (!GRAD && !TRACE && !SMALL), "REC is a variant of the generic untraced forward kernel");
-  static_assert(!FB || (!GRAD && !TRACE && !SMALL && !REC), "FB is a variant of the generic untraced forward kernel");
-  static_assert(!VJP || (GRAD && !TRACE && !SMALL && !REC && !FB), "VJP is a variant of the gradient kernel");
+  static_assert(!FB || (!TRACE && !SMALL && (!GRAD || VJP)), "FB is a variant of the generic untraced forward kernel or of the adjoint kernel");
+  static_assert(!VJP || (GRAD && !TRACE && !SMALL && !REC), "VJP is a variant of the gradient kernel");
   extern __shared__ double arena[];
   __shared__ __align__(8) int s_env[128];  // CTA-wide mailbox, layout: dojo_kernels.cuh (cta_align)
   // a CTA hosts a.slots environments at a time; slot k is served by threads [k * 32 nw, (k + 1) * 32 nw)
@@ -290,11 +440,11 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
     const double* z = a.Z + (size_t)e * P.nz;
     int worst = 0, iters = 0, status = 0;
     if (VJP) {
-      status = rollout_vjp(c, a, e);
+      status = FB ? rollout_feedback_vjp(c, a, e) : rollout_vjp(c, a, e);
     } else if (!GRAD) {
       for (int t = 0; t < a.T; ++t) {
         const double* u = a.U ? a.U + ((size_t)t * a.B + e) * P.nu : nullptr;
-        if (FB) u = feedback(c, a, z, e, t);
+        if (FB) u = feedback<REC>(c, a, z, e, t);
         const double* fx = a.Fext ? a.Fext + (size_t)e * 6 * P.Nb : nullptr;
         prologue(c, z, u, fx, false);
         status = mehrotra<TRACE, SMALL>(c, a.opts, &iters, TRACE ? a.trace + (size_t)e * max(a.opts.max_iter, 0) * 5 : nullptr);
@@ -320,6 +470,12 @@ __global__ void __launch_bounds__(DJ_LB_THREADS, DJ_LB_BLOCKS) dojo_step_kernel(
           }
         }
         if (t + 1 < a.T) { __threadfence_block(); slot_sync(c); z = zo; }
+      }
+      if (REC && FB) {  // x_T = m(z_T), the last slab of the law's states
+        __threadfence_block();
+        slot_sync(c);
+        const double* zT = a.traj + ((size_t)(a.T - 1) * a.B + e) * P.nz;
+        for (int j = c.tid; j < P.Ne; j += c.nthreads) max_to_min_joint(c.joints[j], P.h, zT, a.fb_xtraj + ((size_t)a.T * a.B + e) * 2 * P.nu);
       }
       if (a.traj && !REC) {  // final state also goes to Zn
         slot_sync(c);

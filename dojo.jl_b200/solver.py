@@ -31,7 +31,8 @@ EXPORTS = ["dojo_default_options", "dojo_create", "dojo_destroy", "dojo_last_err
            "dojo_gather_create", "dojo_gather_export", "dojo_gather_connect", "dojo_gather_buffer", "dojo_gather_destroy", "dojo_step_gather_async",
            "dojo_step_grad_gather_async", "dojo_step_trace", "dojo_step_trace_async", "dojo_rollout_grad", "dojo_rollout_grad_async",
            "dojo_rollout_minimal_gradients", "dojo_rollout_feedback", "dojo_rollout_feedback_async", "dojo_lqr_backward", "dojo_lqr_backward_async",
-           "dojo_rollout_tape", "dojo_rollout_tape_async", "dojo_rollout_vjp", "dojo_rollout_vjp_async"]
+           "dojo_rollout_tape", "dojo_rollout_tape_async", "dojo_rollout_vjp", "dojo_rollout_vjp_async",
+           "dojo_rollout_feedback_tape", "dojo_rollout_feedback_tape_async", "dojo_rollout_feedback_vjp", "dojo_rollout_feedback_vjp_async"]
 
 _lib = None
 
@@ -139,6 +140,15 @@ def load_library():
     L.dojo_rollout_feedback.restype = C.c_int
     L.dojo_rollout_feedback_async.argtypes = [vp, op, C.c_int, C.c_int, vp, fp, vp, vp, vp, vp, vp, vp]
     L.dojo_rollout_feedback_async.restype = C.c_int
+    gp = C.POINTER(capi.DojoFeedbackGrad)
+    L.dojo_rollout_feedback_tape.argtypes = [vp, op, C.c_int, C.c_int, vp, fp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_feedback_tape.restype = C.c_int
+    L.dojo_rollout_feedback_tape_async.argtypes = [vp, op, C.c_int, C.c_int, vp, fp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dojo_rollout_feedback_tape_async.restype = C.c_int
+    L.dojo_rollout_feedback_vjp.argtypes = [vp, C.c_int, C.c_int, fp, vp, vp, vp, vp, vp, vp, vp, vp, gp, vp, vp, vp]
+    L.dojo_rollout_feedback_vjp.restype = C.c_int
+    L.dojo_rollout_feedback_vjp_async.argtypes = [vp, C.c_int, C.c_int, fp, vp, vp, vp, vp, vp, vp, vp, vp, gp, vp, vp, vp, vp]
+    L.dojo_rollout_feedback_vjp_async.restype = C.c_int
     cp = C.POINTER(capi.DojoQuadraticCost)
     L.dojo_lqr_backward.argtypes = [vp, C.c_int, C.c_int, cp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.dojo_lqr_backward.restype = C.c_int
@@ -477,6 +487,59 @@ class BatchedStepper:
         self._check(rc, "dojo_rollout_feedback")
         return Zf, st, traj, Ua, xi
 
+    def rollout_feedback_tape(self, Z0, T: int, K, x_ref=None, u_ref=None, K_i=None, xi=None, opts=None):
+        """rollout_feedback recorded for rollout_feedback_vjp (dojo_rollout_feedback_tape); the law's arguments as rollout_feedback.  Returns a
+        dict: Z_traj [T+1, B, 13Nb], X_traj [T+1, B, 2nu] (x_t of the law; slab T = maximal_to_minimal(z_T)), Xi_traj [T, B, 2nu] or None
+        (no K_i), U [T, B, nu] (the applied inputs), tape [T, B, nres], status / iters [T, B], xi [B, 2nu] (after the call) or None."""
+        Z0 = np.ascontiguousarray(np.atleast_2d(Z0), dtype=np.float64)
+        B, T, nx = Z0.shape[0], int(T), 2 * self.nu
+        assert Z0.shape[1] == self.nz
+        steps, envs, Kc, xr, ur, Kic = feedback_arrays(T, B, self.nu, K, x_ref, u_ref, K_i)
+        fb = capi.DojoFeedback(steps, envs, capi.dptr(Kc), None if Kic is None else capi.dptr(Kic), None if xr is None else capi.dptr(xr),
+                               None if ur is None else capi.dptr(ur))
+        xi = None if Kic is None else (np.zeros((B, nx)) if xi is None else np.array(np.broadcast_to(np.asarray(xi, dtype=np.float64), (B, nx))))
+        Tn = max(T, 0)
+        traj, X = np.empty((Tn + 1, B, self.nz)), np.empty((Tn + 1, B, nx))
+        Xi = None if Kic is None else np.empty((Tn, B, nx))
+        Ua, tape = np.empty((Tn, B, self.nu)), np.empty((Tn, B, self.nres))
+        st, it = np.zeros((Tn, B), dtype=np.int32), np.zeros((Tn, B), dtype=np.int32)
+        o = opts if opts is not None else capi.solver_options()
+        rc = self.L.dojo_rollout_feedback_tape(self.h, C.byref(o), B, T, _p(Z0), C.byref(fb), _p(xi), _p(traj), _p(X), _p(Xi), _p(Ua), _p(tape),
+                                               _p(st), _p(it))
+        self._check(rc, "dojo_rollout_feedback_tape")
+        return dict(Z_traj=traj, X_traj=X, Xi_traj=Xi, U=Ua, tape=tape, status=st, iters=it, xi=xi)
+
+    def rollout_feedback_vjp(self, rec, K, x_ref=None, u_ref=None, K_i=None, gZ=None, gX=None, gU=None):
+        """Reverse-mode derivative of the closed loop rollout_feedback_tape recorded (dojo_rollout_feedback_vjp): rec is its dict, the law
+        the same arguments.  Cotangents, each optional: gZ [T+1, B, 12Nb] (packing [x, v, phi, w]), gX [T+1, B, 2nu] on the law's x_t, gU
+        [T, B, nu] on the applied inputs.  Returns a dict: gZ0 [B, 12Nb], gxi0 [B, 2nu] or None, status [B] (0, or 3: that environment's
+        outputs are NaN), and per environment the law gradients K / K_i [steps, B, nu, 2nu], x_ref [steps, B, 2nu], u_ref [steps, B, nu]
+        (steps = 1: the sum over t; a law array shared by the environments gets one gradient per environment)."""
+        tape = np.ascontiguousarray(rec["tape"], dtype=np.float64)
+        T, B = tape.shape[0], tape.shape[1]
+        nu, nx = self.nu, 2 * self.nu
+        steps, envs, Kc, xr, ur, Kic = feedback_arrays(T, B, nu, K, x_ref, u_ref, K_i)
+        fb = capi.DojoFeedback(steps, envs, capi.dptr(Kc), None if Kic is None else capi.dptr(Kic), None if xr is None else capi.dptr(xr),
+                               None if ur is None else capi.dptr(ur))
+        c = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float64)  # noqa: E731
+        Zt, X, Xi, U, gZ, gX, gU = (c(rec["Z_traj"]), c(rec["X_traj"]), c(rec["Xi_traj"]), c(rec["U"]), c(gZ), c(gX), c(gU))
+        assert Zt.shape == (T + 1, B, self.nz) and X.shape == (T + 1, B, nx) and U.shape == (T, B, nu)
+        assert gZ is None or gZ.shape == (T + 1, B, self.ngrad)
+        assert gX is None or gX.shape == (T + 1, B, nx)
+        assert gU is None or gU.shape == (T, B, nu)
+        out = dict(K=np.empty((steps, B, nx, nu)), K_i=None if Kic is None else np.empty((steps, B, nx, nu)), x_ref=np.empty((steps, B, nx)),
+                   u_ref=np.empty((steps, B, nu)))
+        g = capi.DojoFeedbackGrad(*[None if out[k] is None else capi.dptr(out[k]) for k in ("K", "K_i", "x_ref", "u_ref")])
+        gZ0, gxi0 = np.empty((B, self.ngrad)), (None if Kic is None else np.empty((B, nx)))
+        st = np.zeros(B, dtype=np.int32)
+        rc = self.L.dojo_rollout_feedback_vjp(self.h, B, T, C.byref(fb), _p(Zt), _p(X), _p(Xi), _p(U), _p(tape), _p(gZ), _p(gX), _p(gU), C.byref(g),
+                                              _p(gZ0), _p(gxi0), _p(st))
+        self._check(rc, "dojo_rollout_feedback_vjp")
+        res = dict(gZ0=gZ0, gxi0=gxi0, status=st)
+        for k, v in out.items():
+            res[k] = None if v is None else (v.swapaxes(-1, -2) if v.ndim == 4 else v)
+        return res
+
     def lqr_backward(self, X_traj, U, Gx, Gu, cost, mu=None, active=None):
         """Riccati backward pass of iLQR / TVLQR (dojo_lqr_backward) on the shapes rollout_minimal_gradients returns: X_traj [T+1, B, 2nu],
         U [T, B, nu] or None, Gx [T, B, 2nu, 2nu], Gu [T, B, 2nu, nu].  cost has the attributes Q, R, x_goal, u_goal, Q_final,
@@ -751,6 +814,32 @@ class BatchedStepper:
         rc = self.L.dojo_rollout_vjp_async(self.h, int(B), int(T), _p(dZ_traj), _p(dU), _p(dtape), _p(dgZ), _p(dgZ0), _p(dgU), _p(dstatus),
                                            C.c_void_p(int(stream)))
         self._check(rc, "dojo_rollout_vjp_async")
+
+    def rollout_feedback_tape_device(self, dZ0: int, dZ_traj: int, dX_traj: int, dU_applied: int, dtape: int, B: int, T: int, dK: int, steps: int = 1,
+                                     envs: int = 1, dK_i=None, dx_ref=None, du_ref=None, dxi=None, dXi_traj=None, dstatus=None, diters=None, opts=None,
+                                     stream: int = 0):
+        """dojo_rollout_feedback_tape_async on device pointers: the law's arrays as rollout_feedback_device; Z_traj [T+1, B, 13Nb], X_traj
+        [T+1, B, 2nu], Xi_traj [T, B, 2nu] (iff K_i), U_applied [T, B, nu], tape [T, B, nres], status / iters [T, B] (nullable)."""
+        o = opts if opts is not None else capi.solver_options()
+        cp = lambda d: None if d is None else C.cast(C.c_void_p(int(d)), capi.c_double_p)  # noqa: E731
+        fb = capi.DojoFeedback(int(steps), int(envs), cp(dK), cp(dK_i), cp(dx_ref), cp(du_ref))
+        rc = self.L.dojo_rollout_feedback_tape_async(self.h, C.byref(o), int(B), int(T), _p(dZ0), C.byref(fb), _p(dxi), _p(dZ_traj), _p(dX_traj),
+                                                     _p(dXi_traj), _p(dU_applied), _p(dtape), _p(dstatus), _p(diters), C.c_void_p(int(stream)))
+        self._check(rc, "dojo_rollout_feedback_tape_async")
+
+    def rollout_feedback_vjp_device(self, dZ_traj: int, dX_traj: int, dU_applied: int, dtape: int, dgZ0: int, B: int, T: int, dK: int, steps: int = 1,
+                                    envs: int = 1, dK_i=None, dx_ref=None, du_ref=None, dXi_traj=None, dgZ=None, dgX=None, dgU=None, dgK=None,
+                                    dgK_i=None, dgx_ref=None, dgu_ref=None, dgxi0=None, dstatus=None, stream: int = 0):
+        """dojo_rollout_feedback_vjp_async on device pointers: the record of rollout_feedback_tape_device, the cotangents gZ [T+1, B, 12Nb],
+        gX [T+1, B, 2nu], gU [T, B, nu] (nullable), the outputs gZ0 [B, 12Nb], gxi0 [B, 2nu] (with K_i), gK / gK_i [steps, B, 2nu, nu],
+        gx_ref [steps, B, 2nu], gu_ref [steps, B, nu] and status [B] (nullable)."""
+        cp = lambda d: None if d is None else C.cast(C.c_void_p(int(d)), capi.c_double_p)  # noqa: E731
+        fb = capi.DojoFeedback(int(steps), int(envs), cp(dK), cp(dK_i), cp(dx_ref), cp(du_ref))
+        g = capi.DojoFeedbackGrad(cp(dgK), cp(dgK_i), cp(dgx_ref), cp(dgu_ref))
+        rc = self.L.dojo_rollout_feedback_vjp_async(self.h, int(B), int(T), C.byref(fb), _p(dZ_traj), _p(dX_traj), _p(dXi_traj), _p(dU_applied),
+                                                    _p(dtape), _p(dgZ), _p(dgX), _p(dgU), C.byref(g), _p(dgZ0), _p(dgxi0), _p(dstatus),
+                                                    C.c_void_p(int(stream)))
+        self._check(rc, "dojo_rollout_feedback_vjp_async")
 
     def rollout_feedback_device(self, dZ0: int, dZf: int, B: int, T: int, dK: int, steps: int = 1, envs: int = 1, dK_i=None, dx_ref=None, du_ref=None,
                                 dxi=None, dtraj=None, dU_applied=None, dstatus=None, opts=None, stream: int = 0):

@@ -317,6 +317,62 @@ function rollout_vjp(mech::Mechanism, Z_traj::Array{Float64,3}, U::Array{Float64
     rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
     return gZ0, gU, status
 end
+struct CFeedbackGrad  # = DojoFeedbackGrad (include/dojo_b200.h)
+    K::Ptr{Float64}; K_i::Ptr{Float64}; x_ref::Ptr{Float64}; u_ref::Ptr{Float64}
+end
+_fb_layout(mech, nu, K, x_ref, u_ref, K_i) = begin
+    lay(A, tail) = A === nothing ? nothing : reshape(Float64.(A), tail..., size(A, length(tail) + 1), size(A, length(tail) + 2))
+    arrs = (lay(K, (nu, 2nu)), lay(K_i, (nu, 2nu)), lay(x_ref, (2nu,)), lay(u_ref, (nu,)))
+    given = [a for a in arrs if a !== nothing]
+    envs = maximum(size(a, ndims(a) - 1) for a in given); steps = maximum(size(a, ndims(a)) for a in given)
+    full(a) = a === nothing ? nothing : (o = zeros(size(a)[1:end-2]..., envs, steps); o .= a; o)
+    (map(full, arrs)..., steps, envs)
+end
+"rollout_feedback recorded for rollout_feedback_vjp (the law's arguments as rollout_feedback): returns a NamedTuple (Z_traj 13Nb x B x (T+1),
+ X_traj 2nu x B x (T+1) (the law's x_t; slab T+1 = maximal_to_minimal of the last state), Xi_traj 2nu x B x T or nothing (no K_i),
+ U nu x B x T (applied inputs), tape nres x B x T, status B x T, xi); xi is updated in place as by rollout_feedback"
+function rollout_feedback_tape(mech::Mechanism, Z0::Matrix{Float64}, T::Integer, K::AbstractArray; x_ref = nothing, u_ref = nothing,
+                               K_i = nothing, xi = nothing, opts = SolverOptions{Float64}())
+    h = handle(mech); B = size(Z0, 2); nu = h.nu
+    Kf, Kif, xrf, urf, steps, envs = _fb_layout(mech, nu, K, x_ref, u_ref, K_i)
+    (Kif !== nothing && xi === nothing) && (xi = zeros(2nu, B))
+    nres = ccall((:dojo_num_residual, LIB), Cint, (Ptr{Cvoid},), h.ptr)
+    p(a) = a === nothing ? Ptr{Float64}(C_NULL) : pointer(a)
+    traj = zeros(h.nz, B, T + 1); X = zeros(2nu, B, T + 1); Xi = Kif === nothing ? nothing : zeros(2nu, B, T)
+    Ua = zeros(nu, B, T); tape = zeros(nres, B, T); status = zeros(Int32, B, T); iters = zeros(Int32, B, T)
+    rc = GC.@preserve Kf Kif xrf urf Xi begin
+        fb = CFeedback(Int32(steps), Int32(envs), p(Kf), p(Kif), p(xrf), p(urf))
+        ccall((:dojo_rollout_feedback_tape, LIB), Cint,
+              (Ptr{Cvoid}, Ref{COptions}, Cint, Cint, Ptr{Float64}, Ref{CFeedback}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+               Ptr{Float64}, Ptr{Float64}, Ptr{Int32}, Ptr{Int32}),
+              h.ptr, COptions(opts), B, T, Z0, fb, xi === nothing ? C_NULL : xi, traj, X, p(Xi), Ua, tape, status, iters)
+    end
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return (Z_traj = traj, X_traj = X, Xi_traj = Xi, U = Ua, tape = tape, status = status, xi = xi)
+end
+"reverse mode through the closed loop rollout_feedback_tape recorded (rec: its NamedTuple; the law's arguments as there).  Cotangents, each
+ optional: gZ 12Nb x B x (T+1) (packing [x, v, phi, w] per body), gX 2nu x B x (T+1) on x_t, gU nu x B x T on the applied inputs.  Returns
+ (gZ0 12Nb x B, gxi0 2nu x B or nothing, gK nu x 2nu x B x steps, gK_i (or nothing), gx_ref 2nu x B x steps, gu_ref nu x B x steps, status B):
+ the law gradients per environment (a law shared by the environments gets one gradient per environment; sum them)"
+function rollout_feedback_vjp(mech::Mechanism, rec, K::AbstractArray; x_ref = nothing, u_ref = nothing, K_i = nothing, gZ = nothing,
+                              gX = nothing, gU = nothing)
+    h = handle(mech); B = size(rec.Z_traj, 2); T = size(rec.tape, 3); nu = h.nu; ng = 12 * length(mech.bodies)
+    Kf, Kif, xrf, urf, steps, envs = _fb_layout(mech, nu, K, x_ref, u_ref, K_i)
+    p(a) = a === nothing ? Ptr{Float64}(C_NULL) : pointer(a)
+    gZ0 = zeros(ng, B); gxi0 = Kif === nothing ? nothing : zeros(2nu, B)
+    gK = zeros(nu, 2nu, B, steps); gKi = Kif === nothing ? nothing : zeros(nu, 2nu, B, steps)
+    gxr = zeros(2nu, B, steps); gur = zeros(nu, B, steps); status = zeros(Int32, B)
+    rc = GC.@preserve Kf Kif xrf urf gZ gX gU gK gKi gxr gur gxi0 rec begin
+        fb = CFeedback(Int32(steps), Int32(envs), p(Kf), p(Kif), p(xrf), p(urf))
+        out = CFeedbackGrad(p(gK), p(gKi), p(gxr), p(gur))
+        ccall((:dojo_rollout_feedback_vjp, LIB), Cint,
+              (Ptr{Cvoid}, Cint, Cint, Ref{CFeedback}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+               Ptr{Float64}, Ptr{Float64}, Ref{CFeedbackGrad}, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}),
+              h.ptr, B, T, fb, rec.Z_traj, rec.X_traj, p(rec.Xi_traj), rec.U, rec.tape, p(gZ), p(gX), p(gU), out, gZ0, p(gxi0), status)
+    end
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return gZ0, gxi0, gK, gKi, gxr, gur, status
+end
 "the same in minimal coordinates (get_minimal_gradients! at every step): X_traj 2nu x B x (T+1), Gx 2nu x 2nu x B x T, Gu 2nu x nu x B x T"
 function rollout_minimal_gradients(mech::Mechanism, X0::Matrix{Float64}, U::Array{Float64,3}; opts = SolverOptions{Float64}())
     h = handle(mech); B = size(X0, 2); T = size(U, 3); nm = 2 * h.nu

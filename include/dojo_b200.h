@@ -25,6 +25,8 @@
  *   dojo_rollout_minimal_gradients <- simulate! + get_minimal_gradients! at every step
  *   dojo_rollout_tape + dojo_rollout_vjp <- simulate! + get_maximal_gradients! at every step, contracted with a loss gradient
  *                                   (the vector-Jacobian product, without the Jacobians)
+ *   dojo_rollout_feedback_tape + dojo_rollout_feedback_vjp <- the same through dojo_rollout_feedback's closed loop, with the
+ *                                   gradients of the law's gains and references (pendulum_pid.jl's gains tuned by gradient)
  *   dojo_lqr_backward            <- the backward pass of IterativeLQR.jl's solve! (iLQR / TVLQR gains
  *                                   from the minimal-coordinate Jacobians and a quadratic cost;
  *                                   docs/src/examples/trajectory_optimization.md)
@@ -449,6 +451,48 @@ int dojo_rollout_vjp(DojoHandle* h, int B, int T, const double* Z_traj, const do
                      double* gU, int32_t* status);
 int dojo_rollout_vjp_async(DojoHandle* h, int B, int T, const double* dZ_traj, const double* dU, const double* dtape, const double* dgZ,
                            double* dgZ0, double* dgU, int32_t* dstatus, void* cuda_stream);
+
+/* Reverse mode through a closed-loop rollout (dojo_rollout_feedback): gradients of a loss with respect to the law's gains, references
+ * and the initial state, for fitting a controller by gradient (PID / LQR gain tuning, policies linear in the minimal state).
+ * dojo_rollout_feedback_tape is dojo_rollout_feedback recorded like dojo_rollout_tape: Z_traj [13Nb x B x (T+1)] (slab 0 = Z0), the law's
+ * minimal states X_traj [2nu x B x (T+1)] (slab T = maximal_to_minimal(z_T)), its integral states Xi_traj [2nu x B x T] (xi_t, required
+ * if and only if K_i is given), U_applied [nu x B x T], the tape [Nres x B x T], status / iters [B x T] (nullable), and xi in / out as
+ * dojo_rollout_feedback.  Z_traj, U_applied and xi equal dojo_rollout_feedback's bit for bit; Z_traj, the tape, status and iters equal
+ * dojo_rollout_tape(Z0, U_applied)'s.
+ * dojo_rollout_feedback_vjp is its reverse-mode derivative (same fb, Z_traj, X_traj, Xi_traj, U_applied, tape).  With d_t = x_t - x_ref_t,
+ * M_t = dojo_maximal_to_minimal_jacobian at z_t and Fz_t, Fu_t the step Jacobians at the applied inputs (as dojo_rollout_vjp):
+ *   lambda_T = gZ[T] + M_T' gX[T],  nu = 0;  for t = T-1 .. 0:
+ *     a_t = Fu_t' lambda_{t+1} + gUa[t],  nu -= K_i,t' a_t,  d_bar = -K_t' a_t + h nu,
+ *     lambda_t = Fz_t' lambda_{t+1} + gZ[t] + M_t' (d_bar + gX[t]),
+ *     du_ref_t = a_t,  dK_t = -a_t d_t',  dK_i,t = -a_t xi_t',  dx_ref_t = -d_bar;
+ *   gZ0 = lambda_0 [12Nb x B] (required),  gxi0 = nu [2nu x B] (the cotangent of the caller's xi; required with K_i, else not read).
+ * Cotangents, each nullable (= 0): gZ [12Nb x B x (T+1)] in the gradients' packing [x, v, phi, w], gX [2nu x B x (T+1)], gUa [nu x B x T]
+ * on the applied inputs.  The law gradients (DojoFeedbackGrad, nullable, each member nullable) are ALWAYS per environment, [.. x B x steps]
+ * with the DojoFeedback's steps: entry (t, e) at t * B + e; with steps = 1 the sum over t.  A law array shared by all environments
+ * (envs = 1) therefore gets B gradients, which the caller sums: the call has no cross-environment reduction, so every result of an
+ * environment is one lane's fixed-order sum and does not depend on B, the other environments or the launch.  status [B] (nullable): 0, or
+ * 3 if a factorisation was not finite (then every output of that environment is NaN; the others are unaffected).
+ * Both: the checks of dojo_rollout_feedback and of dojo_rollout_tape (DOJO_EINVAL before anything is launched; DOJO_ENOMEM when the
+ * gradient workspace does not fit).  Host or device pointers, all of one kind; the _async forms take device pointers and do not
+ * synchronise. */
+typedef struct {
+  double* K;      /* [nu x 2nu x B x steps], nullable */
+  double* K_i;    /* same shape, nullable (not written without K_i) */
+  double* x_ref;  /* [2nu x B x steps], nullable */
+  double* u_ref;  /* [nu x B x steps], nullable */
+} DojoFeedbackGrad;
+int dojo_rollout_feedback_tape(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* Z0, const DojoFeedback* fb, double* xi,
+                               double* Z_traj, double* X_traj, double* Xi_traj, double* U_applied, double* tape, int32_t* status, int32_t* iters);
+int dojo_rollout_feedback_tape_async(DojoHandle* h, const DojoSolverOptions* opts, int B, int T, const double* dZ0, const DojoFeedback* fb,
+                                     double* dxi, double* dZ_traj, double* dX_traj, double* dXi_traj, double* dU_applied, double* dtape,
+                                     int32_t* dstatus, int32_t* diters, void* cuda_stream);
+int dojo_rollout_feedback_vjp(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* Z_traj, const double* X_traj,
+                              const double* Xi_traj, const double* U_applied, const double* tape, const double* gZ, const double* gX,
+                              const double* gUa, const DojoFeedbackGrad* out, double* gZ0, double* gxi0, int32_t* status);
+int dojo_rollout_feedback_vjp_async(DojoHandle* h, int B, int T, const DojoFeedback* fb, const double* dZ_traj, const double* dX_traj,
+                                    const double* dXi_traj, const double* dU_applied, const double* dtape, const double* dgZ,
+                                    const double* dgX, const double* dgUa, const DojoFeedbackGrad* out, double* dgZ0, double* dgxi0,
+                                    int32_t* dstatus, void* cuda_stream);
 
 /* Batched environment layer (DojoEnvironments/src/environments.jl:77-109 and environments/{ant_ars,quadruped_sampling,
  * pendulum}.jl): state_map / input_map / step! / get_state plus the reward and failure test of the learning examples
