@@ -338,6 +338,31 @@ def get_minimal_trajectory_gradients(mechanism: Mechanism, x0, U, opts=None, dev
     return Xt, Gx, Gu, status
 
 
+def get_minimal_trajectory_vjp(mechanism: Mechanism, x0, U, gX, opts=None, device: int = 0):
+    """The vector-Jacobian product of a rollout in minimal coordinates, without the Jacobians: the rollout from minimal_to_maximal(x0)
+    recorded on the device (dojo_rollout_tape), its states mapped to minimal coordinates, then gZ[t] = M(z_t)' gX[t]
+    (dojo_maximal_to_minimal_vjp), one adjoint pass (dojo_rollout_vjp) and gX0 = N(z_0)' lambda_0 (dojo_minimal_to_maximal_vjp).
+    x0 [2nu], U [T, nu], gX [T+1, 2nu] (the cotangent of every minimal state) -> (X_traj [T+1, 2nu], gX0 [2nu], gU [T, nu], status [T]).
+    This is the exact derivative of the computation X_traj comes from: one maximal rollout read out through maximal_to_minimal.  An
+    environment whose backward pass meets a non-finite factorisation gets status 3 at every step and NaN gradients.  Batched: x0 [B, 2nu],
+    U [T, B, nu], gX [T+1, B, 2nu]."""
+    single, X0, U, T = _trajectory_inputs(x0, U)
+    gX = np.asarray(gX, dtype=float)
+    if single:
+        gX = gX.reshape(gX.shape[0], 1, -1)
+    B = X0.shape[0]
+    s = _stepper(mechanism, B, device)
+    traj, tape, status, _ = s.rollout_tape(s.minimal_to_maximal(X0), U, T, opts)
+    Xt = np.stack([s.maximal_to_minimal(traj[t]) for t in range(T + 1)])
+    gZ = s.maximal_to_minimal_vjp(traj.reshape(-1, s.nz), gX.reshape(-1, s.nmin)).reshape(T + 1, B, s.ngrad)
+    gZ0, gU, vst = s.rollout_vjp(traj, U, tape, gZ)
+    gX0 = s.minimal_to_maximal_vjp(traj[0], gZ0)
+    status = np.where(vst[None, :] != 0, vst[None, :], status)
+    if single:
+        return Xt[:, 0], gX0[0], gU[:, 0], status[:, 0]
+    return Xt, gX0, gU, status
+
+
 def minimal_to_maximal(mechanism: Mechanism, x, device: int = 0):
     """minimal_to_maximal(mechanism, x): x [2 nu] or [B, 2 nu] (per joint [c_tra; c_rot; v_tra; v_rot]) -> z [13 Nb] / [B, 13 Nb]."""
     x = np.asarray(x, dtype=float)
@@ -387,6 +412,24 @@ def minimal_to_maximal_jacobian(mechanism: Mechanism, x, device: int = 0):
     s = _stepper(mechanism, X.shape[0], device)
     J = s.minimal_to_maximal_jacobian(s.minimal_to_maximal(X))
     return J[0] if x.ndim == 1 else J
+
+
+def maximal_to_minimal_vjp(mechanism: Mechanism, z, gx, device: int = 0):
+    """The adjoint of maximal_to_minimal at z: M(z)' gx.  z [13 Nb], gx [2 nu] -> [12 Nb] (attitude-reduced [x, v, phi, w] per body);
+    batched z [B, 13 Nb], gx [B, 2 nu] give [B, 12 Nb]."""
+    z = np.asarray(z, dtype=float)
+    g = _stepper(mechanism, 1, device).maximal_to_minimal_vjp(np.atleast_2d(z), np.atleast_2d(np.asarray(gx, dtype=float)))
+    return g[0] if z.ndim == 1 else g
+
+
+def minimal_to_maximal_vjp(mechanism: Mechanism, x, gz, device: int = 0):
+    """The adjoint of minimal_to_maximal at x: N' gz with N = minimal_to_maximal_jacobian(mechanism, x).  x [2 nu], gz [12 Nb]
+    ([x, v, phi, w] per body) -> [2 nu]; batched x [B, 2 nu], gz [B, 12 Nb] give [B, 2 nu]."""
+    x = np.asarray(x, dtype=float)
+    X = np.atleast_2d(x)
+    s = _stepper(mechanism, X.shape[0], device)
+    g = s.minimal_to_maximal_vjp(s.minimal_to_maximal(X), np.atleast_2d(np.asarray(gz, dtype=float)))
+    return g[0] if x.ndim == 1 else g
 
 
 def get_minimal_gradients(mechanism: Mechanism, x, u, opts=None, device: int = 0):

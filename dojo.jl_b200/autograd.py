@@ -1,5 +1,7 @@
 """PyTorch autograd through a fused rollout: rollout(mechanism, Z0, U) is differentiable with respect to Z0 and U, and
-rollout_feedback(mechanism, Z0, K, ...) through a closed loop with respect to Z0 and the linear law's tensors.
+rollout_feedback(mechanism, Z0, K, ...) through a closed loop with respect to Z0 and the linear law's tensors.  The coordinate maps
+minimal_to_maximal / maximal_to_minimal are differentiable too, so rollout_minimal(mechanism, X0, U) starts from and returns minimal
+states, and rollout_feedback(mechanism, minimal_to_maximal(mechanism, X0), K, ...) backpropagates to a minimal start.
 
     from dojo_jl_b200.autograd import rollout
     Z_traj, status = rollout(mech, Z0, U)           # CUDA fp64: Z0 [B, 13Nb], U [T, B, nu] -> Z_traj [T+1, B, 13Nb], status [T, B]
@@ -127,6 +129,97 @@ def rollout(mechanism: Mechanism, Z0, U, opts=None):
         raise ValueError(f"rollout: Z0 [B, {mechanism.nz}] and U [T, B, {mechanism.nu}] expected, got {tuple(Z0.shape)} and {tuple(U.shape)}")
     s = _stepper(mechanism, Z0.shape[0], Z0.device.index if Z0.device.index is not None else torch.cuda.current_device())
     return _Rollout.apply(Z0, U, s, opts)
+
+
+def _map_functions():
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    def flat(a, k):  # [..., k] -> contiguous [n, k]
+        return a.detach().reshape(-1, k).contiguous()
+
+    class MinimalToMaximal(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, X, stepper):
+            Xc = flat(X, stepper.nmin)
+            n = Xc.shape[0]
+            Z = torch.empty((n, stepper.nz), dtype=torch.float64, device=X.device)
+            stepper.minimal_to_maximal_device(Xc.data_ptr(), Z.data_ptr(), n, stream=torch.cuda.current_stream(X.device).cuda_stream)
+            ctx.save_for_backward(Z)
+            ctx.stepper, ctx.shape = stepper, X.shape
+            return Z.reshape(X.shape[:-1] + (stepper.nz,))
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gZ):
+            (Z,) = ctx.saved_tensors
+            s = ctx.stepper
+            g = to_attitude(Z, gZ.to(torch.float64).reshape(Z.shape)).contiguous()
+            gX = torch.empty((Z.shape[0], s.nmin), dtype=torch.float64, device=Z.device)
+            s.minimal_to_maximal_vjp_device(Z.data_ptr(), g.data_ptr(), gX.data_ptr(), Z.shape[0], stream=torch.cuda.current_stream(Z.device).cuda_stream)
+            return gX.reshape(ctx.shape), None
+
+    class MaximalToMinimal(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, Z, stepper):
+            Zc = flat(Z, stepper.nz)
+            n = Zc.shape[0]
+            X = torch.empty((n, stepper.nmin), dtype=torch.float64, device=Z.device)
+            stepper.maximal_to_minimal_device(Zc.data_ptr(), X.data_ptr(), n, stream=torch.cuda.current_stream(Z.device).cuda_stream)
+            ctx.save_for_backward(Zc)
+            ctx.stepper, ctx.shape = stepper, Z.shape
+            return X.reshape(Z.shape[:-1] + (stepper.nmin,))
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, gX):
+            (Z,) = ctx.saved_tensors
+            s = ctx.stepper
+            g = gX.to(torch.float64).reshape(Z.shape[0], s.nmin).contiguous()
+            gZ = torch.empty((Z.shape[0], s.ngrad), dtype=torch.float64, device=Z.device)
+            s.maximal_to_minimal_vjp_device(Z.data_ptr(), g.data_ptr(), gZ.data_ptr(), Z.shape[0], stream=torch.cuda.current_stream(Z.device).cuda_stream)
+            return from_attitude(Z, gZ).reshape(ctx.shape), None
+
+    return MinimalToMaximal, MaximalToMinimal
+
+
+_MinimalToMaximal = _MaximalToMinimal = None
+
+
+def _map_inputs(mechanism: Mechanism, a, k: int, what: str):
+    import torch
+    global _MinimalToMaximal, _MaximalToMinimal
+    if _MinimalToMaximal is None:
+        _MinimalToMaximal, _MaximalToMinimal = _map_functions()
+    if not torch.is_tensor(a) or a.dtype != torch.float64 or not a.is_cuda:
+        raise ValueError(f"{what}: a float64 CUDA tensor expected")
+    if a.dim() < 1 or a.shape[-1] != k or a.numel() == 0:
+        raise ValueError(f"{what}: [..., {k}] expected, got {tuple(a.shape)}")
+    return _stepper(mechanism, 1, a.device.index if a.device.index is not None else torch.cuda.current_device())
+
+
+def minimal_to_maximal(mechanism: Mechanism, X):
+    """minimal_to_maximal on the current torch stream, differentiable: X [..., 2nu] -> Z [..., 13Nb] (CUDA float64).  The backward pass
+    maps the quaternion cotangents to the attitude packing (to_attitude) and applies N(z)' (dojo_minimal_to_maximal_vjp_async).
+    Once differentiable."""
+    s = _map_inputs(mechanism, X, 2 * mechanism.nu, "minimal_to_maximal")
+    return _MinimalToMaximal.apply(X, s)
+
+
+def maximal_to_minimal(mechanism: Mechanism, Z):
+    """maximal_to_minimal on the current torch stream, differentiable: Z [..., 13Nb] -> X [..., 2nu] (CUDA float64).  The backward pass
+    applies M(z)' (dojo_maximal_to_minimal_vjp_async) and returns the quaternion part as G(q) phibar (from_attitude), tangent to the unit
+    sphere as in rollout().  Once differentiable."""
+    s = _map_inputs(mechanism, Z, mechanism.nz, "maximal_to_minimal")
+    return _MaximalToMinimal.apply(Z, s)
+
+
+def rollout_minimal(mechanism: Mechanism, X0, U, opts=None):
+    """rollout() in minimal coordinates: maximal_to_minimal(rollout(minimal_to_maximal(X0), U)), differentiable with respect to
+    X0 [B, 2nu] and U [T, B, nu].  Returns (X_traj [T+1, B, 2nu], status [T, B]).  The gradients are the exact derivative of this
+    computation: one maximal rollout from minimal_to_maximal(X0), read out through maximal_to_minimal."""
+    Z_traj, status = rollout(mechanism, minimal_to_maximal(mechanism, X0), U, opts)
+    return maximal_to_minimal(mechanism, Z_traj), status
 
 
 def _feedback_function():

@@ -1550,6 +1550,76 @@ static int kinjac_sync(DojoHandle* h, int mode, int B, const double* Z, double* 
 extern "C" int dojo_maximal_to_minimal_jacobian(DojoHandle* h, int B, const double* Z, double* J) { return kinjac_sync(h, 0, B, Z, J, "dojo_maximal_to_minimal_jacobian"); }
 extern "C" int dojo_minimal_to_maximal_jacobian(DojoHandle* h, int B, const double* Z, double* J) { return kinjac_sync(h, 1, B, Z, J, "dojo_minimal_to_maximal_jacobian"); }
 
+// ------------------------------------------------------------------------------------------------------------
+// Adjoints of the coordinate maps: gZ = M(z)' gX and gX = N(z)' gZ without forming M or N (dojo_kinjac.cuh)
+// ------------------------------------------------------------------------------------------------------------
+static int map_vjp_check(DojoHandle* h, int n, bool buffers, const char* who) {
+  if (!h) return DOJO_EINVAL;
+  if (n <= 0 || !buffers || h->plan.nu == 0) { h->err = std::string(who) + ": bad arguments (n >= 1, every buffer, a mechanism with inputs)"; return DOJO_EINVAL; }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  return DOJO_OK;
+}
+
+// to_minimal: gZ = M' gX (in = gX, out = gZ);  else gX = N' gZ (in = gZ, out = gX)
+static int launch_map_vjp(DojoHandle* h, bool to_minimal, int n, const double* dZ, const double* din, double* dout, cudaStream_t s) {
+  const Plan& P = h->plan;
+  MapVjpArgs a;
+  a.joints = P.joints; a.order = h->d_kin_order;
+  a.Ne = P.Ne; a.Nb = P.Nb; a.nu = P.nu; a.n = n; a.h = P.h;
+  a.Z = dZ; a.in = din; a.out = dout; a.ws = nullptr;
+  if (to_minimal) {
+    int G = 1;  // lanes per state: the joints and the bodies each take one lane, up to a warp
+    while (G < 32 && (G < P.Ne || G < P.Nb)) G *= 2;
+    int per_cta = 128 / G;
+    const size_t per_state = (size_t)24 * P.Ne * sizeof(double);
+    while (per_cta > 1 && per_cta * per_state > 48 * 1024) per_cta /= 2;
+    const size_t smem = per_cta * per_state;
+    if (smem > 48 * 1024) CUDA_TRY(h, cudaFuncSetAttribute(dojo_max_to_min_vjp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    enter_call(h, s);
+    dojo_max_to_min_vjp_kernel<<<(n + per_cta - 1) / per_cta, per_cta * G, smem, s>>>(a, G);
+  } else {
+    int rc = ensure_kinjac(h);  // its per-CTA slices hold kinjac_ws_doubles >= min_to_max_vjp_ws_doubles doubles (nu >= 1)
+    if (rc != DOJO_OK) return rc;
+    a.ws = h->d_kjws;
+    enter_call(h, s);
+    dojo_min_to_max_vjp_kernel<<<std::min(n, h->kj_grid), 32, 0, s>>>(a);
+  }
+  CUDA_TRY(h, cudaGetLastError());
+  h->launches += 1;
+  leave_call(h, s);
+  return DOJO_OK;
+}
+
+extern "C" int dojo_maximal_to_minimal_vjp_async(DojoHandle* h, int n, const double* dZ, const double* dgX, double* dgZ, void* cuda_stream) {
+  const int rc = map_vjp_check(h, n, dZ && dgX && dgZ, "dojo_maximal_to_minimal_vjp_async");
+  return rc != DOJO_OK ? rc : launch_map_vjp(h, true, n, dZ, dgX, dgZ, (cudaStream_t)cuda_stream);
+}
+extern "C" int dojo_minimal_to_maximal_vjp_async(DojoHandle* h, int n, const double* dZ, const double* dgZ, double* dgX, void* cuda_stream) {
+  const int rc = map_vjp_check(h, n, dZ && dgZ && dgX, "dojo_minimal_to_maximal_vjp_async");
+  return rc != DOJO_OK ? rc : launch_map_vjp(h, false, n, dZ, dgZ, dgX, (cudaStream_t)cuda_stream);
+}
+
+// host or device pointers (all of the same kind); n is not bounded by max_batch: host arrays are staged whole through the arena
+static int map_vjp_sync(DojoHandle* h, bool to_minimal, int n, const double* Z, const double* in, double* out, const char* who) {
+  int rc = map_vjp_check(h, n, Z && in && out, who);
+  if (rc != DOJO_OK) return rc;
+  const Plan& P = h->plan;
+  const size_t nx = (size_t)n * 2 * P.nu, ng = (size_t)n * 12 * P.Nb;
+  const double *dZ = Z, *din = in;
+  double* dout = out;
+  HostCall c(h, Z);
+  c.in(&dZ, (size_t)n * P.nz); c.in(&din, to_minimal ? nx : ng); c.out(&dout, to_minimal ? ng : nx);
+  rc = c.bind();
+  if (rc == DOJO_OK) rc = launch_map_vjp(h, to_minimal, n, dZ, din, dout, h->stream);
+  return c.finish(rc);
+}
+extern "C" int dojo_maximal_to_minimal_vjp(DojoHandle* h, int n, const double* Z, const double* gX, double* gZ) {
+  return map_vjp_sync(h, true, n, Z, gX, gZ, "dojo_maximal_to_minimal_vjp");
+}
+extern "C" int dojo_minimal_to_maximal_vjp(DojoHandle* h, int n, const double* Z, const double* gZ, double* gX) {
+  return map_vjp_sync(h, false, n, Z, gZ, gX, "dojo_minimal_to_maximal_vjp");
+}
+
 // get_minimal_gradients! (gradients/state.jl:182-217).  Per chunk of environments, on one stream: minimal -> maximal,
 // forward + gradient kernels (dojo_step_grad_async), the map-Jacobian kernel in mode 2, maximal -> minimal of the next state.
 extern "C" int dojo_minimal_gradients(DojoHandle* h, const DojoSolverOptions* opts, int B, const double* X, const double* U, double* X_next, double* Gx,

@@ -401,6 +401,91 @@ DJ_DEV void kinjac_env(const KinJacArgs& a, int e, double* ws, int tid, int nthr
   }
 }
 
+// ------------------------------------------------------------------------------------------------ adjoints of the two maps
+// Reverse mode through the maps without forming M or N (dojo_maximal_to_minimal_vjp / dojo_minimal_to_maximal_vjp):
+//   gZ = M(z)' gX   [12 Nb] <- [2 nu]      gX = N(z)' gZ   [2 nu] <- [12 Nb]
+// n states, layouts [feature x n]; every output entry is one lane's sum in a fixed order, so a state's result does not depend on n,
+// the grid or the other states.
+struct MapVjpArgs {
+  const JointDev* joints;
+  const int* order;   // joints root -> leaves
+  int Ne, Nb, nu, n;
+  double h;
+  const double* Z;    // [13 Nb x n] the maximal states (for N': minimal_to_maximal(X))
+  const double* in;   // M': gX [2 nu x n]    N': gZ [12 Nb x n], packing [x, v, phi, w] per body
+  double* out;        // M': gZ [12 Nb x n]   N': gX [2 nu x n]
+  double* ws;         // N': per-CTA workspace, min_to_max_vjp_ws_doubles() each
+};
+
+#ifdef __CUDACC__
+__host__ __device__
+#endif
+inline size_t min_to_max_vjp_ws_doubles(int Nb) { return (size_t)300 * Nb; }  // Pm, Pp [Nb][144], the accumulators [12 Nb]
+
+// gZ = M(z)' gX for state e: the closed-loop adjoint's two routines (add_max_to_min_vjp), one lane per joint, then one lane per body.
+// s: [24 Ne] scratch of this state's lanes.
+template <class Sync>
+DJ_DEV void max_to_min_vjp_env(const MapVjpArgs& a, int e, double* s, int tid, int nthr, Sync sync) {
+  const double* z = a.Z + (size_t)e * 13 * a.Nb;
+  const double* w = a.in + (size_t)e * 2 * a.nu;
+  for (int j = tid; j < a.Ne; j += nthr) {
+    const JointDev& jd = a.joints[j];
+    if (jd.nfree_t + jd.nfree_r > 0) max_to_min_vjp_joint(jd, kin_load(z, jd.parent), kin_load(z, jd.child), a.h, w + 2 * jd.u_off, s + (size_t)24 * j);
+  }
+  sync();
+  double* gz = a.out + (size_t)e * 12 * a.Nb;
+  for (int b = tid; b < a.Nb; b += nthr) {
+    double g[12];
+    max_to_min_vjp_fold(a.joints, a.Ne, b, s, g);
+    for (int k = 0; k < 12; ++k) gz[12 * b + k] = g[k];
+  }
+}
+
+// gX = N(z)' gZ for state e: the transpose of kinjac_env's phase-2 chain N_i = Pm_i E_j + Pp_i N_parent(i).  Phase 1 evaluates the
+// partials exactly as kinjac_env does; phase 2 walks the joints leaves -> root (the reverse of `order`) with one accumulator per body:
+//   gbar_i = gZ_i + sum over the children c of i of Pp_c' gbar_c,    gX[joint of child i] = Pm_i[:, :2 nu_j]' gbar_i.
+// A body's accumulator is complete when its own joint is reached, since every joint of which it is the parent comes later in `order`.
+// One barrier per joint; lanes take the joint's 2 nu_j + 12 outputs.
+template <class Sync>
+DJ_DEV void min_to_max_vjp_env(const MapVjpArgs& a, int e, double* ws, int tid, int nthr, Sync sync) {
+  const int Nb = a.Nb, Ne = a.Ne;
+  double* Pm = ws;                      // [Nb][144]
+  double* Pp = Pm + (size_t)144 * Nb;   // [Nb][144]
+  double* gb = Pp + (size_t)144 * Nb;   // [12 Nb]
+  const double* z = a.Z + (size_t)e * 13 * Nb;
+  const double* gz = a.in + (size_t)e * 12 * Nb;
+  double* gx = a.out + (size_t)e * 2 * a.nu;
+  for (int t = tid; t < Ne; t += nthr) {
+    const JointDev& jd = a.joints[t];
+    const BodyState A = kin_load(z, jd.parent), Bc = kin_load(z, jd.child);
+    double xm[12];
+    joint_minimal(jd, A, Bc, a.h, xm);
+    min_to_max_partials(jd, A, Bc.q, xm, a.h, Pm + (size_t)144 * jd.child, Pp + (size_t)144 * jd.child);
+  }
+  for (int k = tid; k < 12 * Nb; k += nthr) gb[k] = gz[k];
+  sync();
+  for (int k = Ne - 1; k >= 0; --k) {
+    const JointDev& jd = a.joints[a.order[k]];
+    const int i = jd.child, p = jd.parent, m = 2 * (jd.nfree_t + jd.nfree_r), c0 = 2 * jd.u_off;
+    const double* pm = Pm + (size_t)144 * i;
+    const double* pp = Pp + (size_t)144 * i;
+    const double* gi = gb + 12 * i;
+    for (int t = tid; t < m + 12; t += nthr) {
+      if (t < m) {
+        double acc = 0.0;
+        for (int r = 0; r < 12; ++r) acc += pm[r * 12 + t] * gi[r];
+        gx[c0 + t] = acc;
+      } else if (p >= 0) {
+        const int q = t - m;
+        double acc = gb[12 * p + q];
+        for (int r = 0; r < 12; ++r) acc += pp[r * 12 + q] * gi[r];
+        gb[12 * p + q] = acc;
+      }
+    }
+    sync();
+  }
+}
+
 #if defined(DJ_HOSTEMU) || (defined(__CUDACC__) && !defined(DJ_ANY_CONTACT))  // dojo_b200_cm.cu includes the routines above only
 // persistent grid: CTA b takes environments b, b + gridDim.x, ...; workspace slice b
 __global__ void __launch_bounds__(128) dojo_kinjac_kernel(const KinJacArgs a) {
@@ -409,6 +494,28 @@ __global__ void __launch_bounds__(128) dojo_kinjac_kernel(const KinJacArgs a) {
     kinjac_env(a, e, ws, (int)threadIdx.x, (int)blockDim.x, [] { __syncthreads(); });
     __syncthreads();  // the workspace is reused by the next environment
   }
+}
+
+// M': a group of G lanes (a power of two <= 32, inside one warp) per state, blockDim.x / G states per CTA, one state per group; the
+// dynamic shared memory holds the [24 Ne] scratch of every group.  Groups never wait for each other.
+__global__ void __launch_bounds__(128) dojo_max_to_min_vjp_kernel(const MapVjpArgs a, int G) {
+#ifdef DJ_HOSTEMU
+  double* smem = hostemu_smem();
+#else
+  extern __shared__ double smem[];
+#endif
+  const int g = (int)threadIdx.x / G, lane = (int)threadIdx.x % G;
+  const int e = (int)blockIdx.x * ((int)blockDim.x / G) + g;
+  if (e >= a.n) return;
+  const unsigned mask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << ((threadIdx.x & 31) & ~(unsigned)(G - 1));
+  max_to_min_vjp_env(a, e, smem + (size_t)g * 24 * a.Ne, lane, G, [mask] { __syncwarp(mask); });
+}
+
+// N': one warp per state, persistent grid: CTA b takes states b, b + gridDim.x, ...; workspace slice b (global memory, L2 resident)
+__global__ void __launch_bounds__(32) dojo_min_to_max_vjp_kernel(const MapVjpArgs a) {
+  double* ws = a.ws + (size_t)blockIdx.x * min_to_max_vjp_ws_doubles(a.Nb);
+  for (int e = blockIdx.x; e < a.n; e += gridDim.x)
+    min_to_max_vjp_env(a, e, ws, (int)threadIdx.x, (int)blockDim.x, [] { __syncwarp(); });  // ends with a barrier: ws is free again
 }
 #endif
 

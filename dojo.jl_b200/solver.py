@@ -32,7 +32,8 @@ EXPORTS = ["dojo_default_options", "dojo_create", "dojo_destroy", "dojo_last_err
            "dojo_step_grad_gather_async", "dojo_step_trace", "dojo_step_trace_async", "dojo_rollout_grad", "dojo_rollout_grad_async",
            "dojo_rollout_minimal_gradients", "dojo_rollout_feedback", "dojo_rollout_feedback_async", "dojo_lqr_backward", "dojo_lqr_backward_async",
            "dojo_rollout_tape", "dojo_rollout_tape_async", "dojo_rollout_vjp", "dojo_rollout_vjp_async",
-           "dojo_rollout_feedback_tape", "dojo_rollout_feedback_tape_async", "dojo_rollout_feedback_vjp", "dojo_rollout_feedback_vjp_async"]
+           "dojo_rollout_feedback_tape", "dojo_rollout_feedback_tape_async", "dojo_rollout_feedback_vjp", "dojo_rollout_feedback_vjp_async",
+           "dojo_maximal_to_minimal_vjp", "dojo_maximal_to_minimal_vjp_async", "dojo_minimal_to_maximal_vjp", "dojo_minimal_to_maximal_vjp_async"]
 
 _lib = None
 
@@ -90,6 +91,11 @@ def load_library():
         getattr(L, name).argtypes = [vp, C.c_int, vp, vp]
         getattr(L, name).restype = C.c_int
         getattr(L, name + "_async").argtypes = [vp, C.c_int, vp, vp, vp]
+        getattr(L, name + "_async").restype = C.c_int
+    for name in ("dojo_maximal_to_minimal_vjp", "dojo_minimal_to_maximal_vjp"):
+        getattr(L, name).argtypes = [vp, C.c_int, vp, vp, vp]
+        getattr(L, name).restype = C.c_int
+        getattr(L, name + "_async").argtypes = [vp, C.c_int, vp, vp, vp, vp]
         getattr(L, name + "_async").restype = C.c_int
     L.dojo_minimal_gradients.argtypes = [vp, op, C.c_int, vp, vp, vp, vp, vp, vp, vp]
     L.dojo_minimal_gradients.restype = C.c_int
@@ -615,6 +621,26 @@ class BatchedStepper:
         self._check(self.L.dojo_minimal_to_maximal_jacobian(self.h, Z.shape[0], _p(Z), _p(J)), "dojo_minimal_to_maximal_jacobian")
         return np.transpose(J, (0, 2, 1))
 
+    def maximal_to_minimal_vjp(self, Z, gX):
+        """The adjoint of maximal_to_minimal (dojo_maximal_to_minimal_vjp): gZ = M(z)' gX per state, Z [n, 13 Nb], gX [n, 2 nu] ->
+        gZ [n, 12 Nb] in the gradients' packing [x, v, phi, w] per body.  n is not bounded by max_batch."""
+        Z = np.ascontiguousarray(np.atleast_2d(Z), dtype=np.float64)
+        gX = np.ascontiguousarray(np.atleast_2d(gX), dtype=np.float64)
+        assert Z.shape[1] == self.nz and gX.shape == (Z.shape[0], self.nmin)
+        gZ = np.empty((Z.shape[0], self.ngrad))
+        self._check(self.L.dojo_maximal_to_minimal_vjp(self.h, Z.shape[0], _p(Z), _p(gX), _p(gZ)), "dojo_maximal_to_minimal_vjp")
+        return gZ
+
+    def minimal_to_maximal_vjp(self, Z, gZ):
+        """The adjoint of minimal_to_maximal (dojo_minimal_to_maximal_vjp): gX = N(z)' gZ per state, at the maximal states Z [n, 13 Nb]
+        (= minimal_to_maximal(X)), gZ [n, 12 Nb] ([x, v, phi, w] per body) -> gX [n, 2 nu].  n is not bounded by max_batch."""
+        Z = np.ascontiguousarray(np.atleast_2d(Z), dtype=np.float64)
+        gZ = np.ascontiguousarray(np.atleast_2d(gZ), dtype=np.float64)
+        assert Z.shape[1] == self.nz and gZ.shape == (Z.shape[0], self.ngrad)
+        gX = np.empty((Z.shape[0], self.nmin))
+        self._check(self.L.dojo_minimal_to_maximal_vjp(self.h, Z.shape[0], _p(Z), _p(gZ), _p(gX)), "dojo_minimal_to_maximal_vjp")
+        return gX
+
     def minimal_gradients(self, X, U=None, opts=None):
         """get_minimal_gradients! (gradients/state.jl:182-217), batched.
         Returns (X_next [B, 2nu], dx'/dx [B, 2nu, 2nu], dx'/du [B, 2nu, nu], status, iters)."""
@@ -769,6 +795,16 @@ class BatchedStepper:
 
     def minimal_to_maximal_jacobian_device(self, dZ: int, dJ: int, B: int, stream: int = 0):
         self._check(self.L.dojo_minimal_to_maximal_jacobian_async(self.h, int(B), _p(dZ), _p(dJ), C.c_void_p(int(stream))), "dojo_minimal_to_maximal_jacobian_async")
+
+    def maximal_to_minimal_vjp_device(self, dZ: int, dgX: int, dgZ: int, n: int, stream: int = 0):
+        """dojo_maximal_to_minimal_vjp_async on device pointers: Z [n, 13Nb], gX [n, 2nu] in, gZ [n, 12Nb] out."""
+        self._check(self.L.dojo_maximal_to_minimal_vjp_async(self.h, int(n), _p(dZ), _p(dgX), _p(dgZ), C.c_void_p(int(stream))),
+                    "dojo_maximal_to_minimal_vjp_async")
+
+    def minimal_to_maximal_vjp_device(self, dZ: int, dgZ: int, dgX: int, n: int, stream: int = 0):
+        """dojo_minimal_to_maximal_vjp_async on device pointers: Z [n, 13Nb], gZ [n, 12Nb] in, gX [n, 2nu] out."""
+        self._check(self.L.dojo_minimal_to_maximal_vjp_async(self.h, int(n), _p(dZ), _p(dgZ), _p(dgX), C.c_void_p(int(stream))),
+                    "dojo_minimal_to_maximal_vjp_async")
 
     def minimal_gradients_device(self, dX: int, dU: Optional[int], dXn: int, dGx: int, dGu: int, B: int, opts=None, dstatus=None, diters=None):
         """device-resident get_minimal_gradients! (synchronises the handle's stream before returning)"""

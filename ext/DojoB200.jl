@@ -317,6 +317,27 @@ function rollout_vjp(mech::Mechanism, Z_traj::Array{Float64,3}, U::Array{Float64
     rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
     return gZ0, gU, status
 end
+"adjoint of maximal_to_minimal: gZ = M(z)' gX per state, Z 13Nb x n, gX 2nu x n -> gZ 12Nb x n (packing [x, v, phi, w] per body); n
+ counts states (a trajectory's B (T+1) slabs go in one call)"
+function maximal_to_minimal_vjp(mech::Mechanism, Z::AbstractMatrix{Float64}, gX::AbstractMatrix{Float64})
+    h = handle(mech); n = size(Z, 2)
+    gZ = zeros(12 * length(mech.bodies), n)
+    rc = ccall((:dojo_maximal_to_minimal_vjp, LIB), Cint, (Ptr{Cvoid}, Cint, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+               h.ptr, n, Matrix{Float64}(Z), Matrix{Float64}(gX), gZ)
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return gZ
+end
+"adjoint of minimal_to_maximal: gX = N(z)' gZ per state at the maximal states Z = minimal_to_maximal(X) (13Nb x n), gZ 12Nb x n -> gX 2nu x n.
+ Reverse mode through a rollout from a minimal start: rollout_tape from minimal_to_maximal(X0), gZ[t] = maximal_to_minimal_vjp(z_t, gX[t]),
+ rollout_vjp, then gX0 = minimal_to_maximal_vjp(z_0, gZ0)"
+function minimal_to_maximal_vjp(mech::Mechanism, Z::AbstractMatrix{Float64}, gZ::AbstractMatrix{Float64})
+    h = handle(mech); n = size(Z, 2)
+    gX = zeros(2 * h.nu, n)
+    rc = ccall((:dojo_minimal_to_maximal_vjp, LIB), Cint, (Ptr{Cvoid}, Cint, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+               h.ptr, n, Matrix{Float64}(Z), Matrix{Float64}(gZ), gX)
+    rc == 0 || error(unsafe_string(ccall((:dojo_last_error, LIB), Cstring, (Ptr{Cvoid},), h.ptr)))
+    return gX
+end
 struct CFeedbackGrad  # = DojoFeedbackGrad (include/dojo_b200.h)
     K::Ptr{Float64}; K_i::Ptr{Float64}; x_ref::Ptr{Float64}; u_ref::Ptr{Float64}
 end

@@ -397,6 +397,22 @@ int dojo_minimal_to_maximal_jacobian(DojoHandle* h, int B, const double* Z, doub
 int dojo_maximal_to_minimal_jacobian_async(DojoHandle* h, int B, const double* dZ, double* dJ, void* cuda_stream);
 int dojo_minimal_to_maximal_jacobian_async(DojoHandle* h, int B, const double* dZ, double* dJ, void* cuda_stream);
 
+/* Adjoints (vector-Jacobian products) of the two maps, without forming the Jacobians above:
+ *   dojo_maximal_to_minimal_vjp   gZ = M(z)' gX   gX [2 nu x n] -> gZ [12 Nb x n]
+ *   dojo_minimal_to_maximal_vjp   gX = N(z)' gZ   gZ [12 Nb x n] -> gX [2 nu x n]
+ * Z [13 Nb x n] is the maximal state; for dojo_minimal_to_maximal_vjp it is minimal_to_maximal(X), as for
+ * dojo_minimal_to_maximal_jacobian.  gZ is in the gradients' packing [x, v, phi, w] per body.  The output is overwritten, not
+ * accumulated.  n counts states, not environments, and is not bounded by max_batch: a trajectory [.. x B x (T+1)] goes in one call
+ * with n = B (T+1).  Each state's result is one fixed-order sum per entry: it does not depend on n or on the other states.
+ * Reverse mode through a rollout in minimal coordinates composes these with the rollout tape and adjoint (INTEGRATION.md):
+ *   z0 = minimal_to_maximal(X0), tape, gZ[t] = M(z_t)' gX[t], dojo_rollout_vjp, gX0 = N(z0)' gZ0.
+ * DOJO_EINVAL, before anything is launched, for n <= 0, a null buffer or a mechanism without inputs (nu = 0).
+ * Host or device pointers (all of the same kind); *_async: device pointers, no synchronisation. */
+int dojo_maximal_to_minimal_vjp(DojoHandle* h, int n, const double* Z, const double* gX, double* gZ);
+int dojo_maximal_to_minimal_vjp_async(DojoHandle* h, int n, const double* dZ, const double* dgX, double* dgZ, void* cuda_stream);
+int dojo_minimal_to_maximal_vjp(DojoHandle* h, int n, const double* Z, const double* gZ, double* gX);
+int dojo_minimal_to_maximal_vjp_async(DojoHandle* h, int n, const double* dZ, const double* dgZ, double* dgX, void* cuda_stream);
+
 /* get_minimal_gradients!(mechanism, x, u; opts)  src/gradients/state.jl:182-217: step_minimal_coordinates! and
  *   Gx = M(z') Fz N(z) [2 nu x 2 nu x B],  Gu = M(z') Fu [2 nu x nu x B]   (column-major per environment),
  * with z = minimal_to_maximal(x), (z', Fz, Fu) = dojo_step_grad(z, u) (consistent IFT, SURVEY Q2), M / N the two map
